@@ -3,9 +3,10 @@
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K --warmup W   # reference CPU arithmetic (rank 0)
+    python bench.py --gpus 1 --steps K --warmup W --dump-outputs DIR # also write the last timed step's outputs as .npy
 
 Workload (config.workload): synthetic 1.3M cells x 2000 HVGs CSR (~5 % dense), n_pcs=50, k=15 — the
-configuration BASELINE.json's metric is quoted on; it fits one B200.  One "step" = one full pass of the
+configuration BASELINE.json's metric is quoted on; it fits one H100 (80 GB).  One "step" = one full pass of the
 hot path over that matrix.  `value` = cells/s with the CSR already resident in HBM (CUDA events on the
 launching stream, barrier + synchronize on both sides, max over ranks); `e2e` = the same pass through
 the public scanpy-signature API (sb.pp.pca / sb.pp.neighbors / sb.tl.leiden) from HOST arrays, all
@@ -52,7 +53,12 @@ def parse_args():
     p.add_argument("--knn-queries", type=int, default=8192)
     p.add_argument("--no-e2e", action="store_true")
     p.add_argument("--no-parity", action="store_true", help="skip the host-side fp64 parity checks after the timed region")
-    return p.parse_args()
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write what the last timed step computed to DIR/<name>.npy (float32/float64, a fixed sample of rows)")
+    a = p.parse_args()
+    if a.steps < 1:
+        p.error("--steps must be >= 1")
+    return a
 
 
 def workload_config(a, n_gpus):
@@ -60,7 +66,7 @@ def workload_config(a, n_gpus):
                          f"n_pcs={a.n_pcs} k={a.k} (BASELINE.json configs[2]{'/[3]' if n_gpus > 1 else ''})",
                 n_cells=a.n_cells, n_genes=a.n_genes, n_pcs=a.n_pcs, n_neighbors=a.k, leiden="resolution=1, n_iterations=-1",
                 parallelism=f"row-sharded x{n_gpus}" if n_gpus > 1 else "single GPU",
-                l2="inputs (1.0 GB CSR, 260 MB X_pca) exceed the 126 MB L2; no explicit flush")
+                l2="inputs (1.0 GB CSR, 260 MB X_pca) exceed the L2 (50 MB on an H100); no explicit flush")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -232,6 +238,45 @@ def parity_checks(a, out, x_host, labels, row_range, n_rows_sample: int = 2000):
 
 
 # ------------------------------------------------------------------------------------------------
+DUMP_ROWS = 32768       # rows of the per-row outputs written by --dump-outputs (a fixed sample: the whole step is ~400 MB)
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, out, n):
+    """What the timed path hands a caller, from its last timed step: the leiden membership of every cell, and X_pca, the
+    kNN lists (self first, as sb2_knn_l2_f32 returns them) and the connectivities CSR rows of a fixed sample of cells
+    (RandomState(0), sorted).  Integers are written as float64 (exact); everything else keeps its float32 / float64."""
+    from scanpy_b200 import _ops
+
+    rows = np.sort(np.random.RandomState(0).choice(n, min(n, DUMP_ROWS), replace=False))
+    indptr, indices, data = (_ops._to_host(t) for t in out["conn"])
+    lo, hi = indptr[rows].astype(np.int64), indptr[rows + 1].astype(np.int64)
+    take = np.concatenate([np.arange(a, b) for a, b in zip(lo, hi)]) if len(rows) else np.zeros(0, np.int64)
+    arrays = dict(
+        sample_rows=rows.astype(np.float64),
+        X_pca=_ops._to_host(out["X_pca"])[rows],
+        pca_variance=np.asarray(out["pca"]["variance"], dtype=np.float64),
+        knn_indices=_ops._to_host(out["knn_idx"])[rows].astype(np.float64),
+        knn_distances=_ops._to_host(out["knn_dist"])[rows],
+        connectivities_indptr=np.concatenate([[0], np.cumsum(hi - lo)]).astype(np.float64),
+        connectivities_indices=indices[take].astype(np.float64),
+        connectivities_data=data[take],
+        leiden_membership=_ops._to_host(out["membership"]).astype(np.float64),
+        modularity=np.array([out["modularity"]], dtype=np.float64),
+    )
+    for k, v in arrays.items():
+        if v.dtype not in (np.float32, np.float64):
+            arrays[k] = v.astype(np.float64)
+    total = sum(v.nbytes for v in arrays.values())
+    if total > DUMP_MAX_BYTES:
+        raise RuntimeError(f"--dump-outputs would write {total} bytes (limit {DUMP_MAX_BYTES})")
+    os.makedirs(out_dir, exist_ok=True)
+    for k, v in arrays.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), v)
+    note(f"dumped {len(arrays)} arrays ({total / 2**20:.1f} MiB) to {out_dir}")
+
+
+# ------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -315,6 +360,8 @@ def run_b200(a, rank, world, local_rank):
         ms_total = float(t.item())
     ms_step = ms_total / a.steps
     value = n / (ms_step / 1e3)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, out, n)
 
     # ---- e2e through the public API from host arrays: every step copies its inputs host -> device (from page-locked
     # host memory, as the contract prescribes) and its results device -> host inside the timed region ----
@@ -380,30 +427,28 @@ def run_b200(a, rank, world, local_rank):
     ki = out["knn_info"]
     ach = ki["pass1_flops"] / (ki["pass1_ms"] * 1e-3) / 1e12
     issued = ki["pass1_issued_flops"] / (ki["pass1_ms"] * 1e-3) / 1e12
-    peak_tensor = peaks.get("bf16_tflops_sustained", 1400.0)
-    sm_max = (clocks or {}).get("sm_max_mhz") or 1965.0
+    peak_tensor = peaks.get("bf16_tflops_sustained", 989.0)
+    sm_max = (clocks or {}).get("sm_max_mhz") or 1980.0
     if ki["pass1_tensor"]:
-        # DRAM bytes per launch of the dominant kernel from the committed ncu capture of this exact workload
-        # (profiles/r1_ncu_metrics_knn_tiered.txt: dram__bytes_read 12.388 GB + dram__bytes_write 0.780 GB)
-        traffic = 11.973e9 if (world == 1 and a.n_cells == 1_300_000 and a.n_pcs == 50 and a.k == 15) else None
-        roofline = dict(bound="tensor", kernel="knn_pass1_tc_kernel", achieved=ach, peak=peak_tensor, unit="TFLOP/s",
-                        frac=ach / peak_tensor, traffic=traffic,
-                        traffic_source=("profiles/r2_ncu_metrics_knn_sweep2_meanfront.txt (ncu --set full of knn_sweep2_kernel, main launch, dram read + write; algorithmic operand bytes: "
-                                        "0.33 GB of fp16 images)" if traffic else None),
-                        peak_source=("MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)" if peaks else "fallback 1.4 PFLOP/s sustained"),
+        roofline = dict(bound="tensor", kernel="knn_sweep2_kernel", achieved=ach, peak=peak_tensor, unit="TFLOP/s",
+                        frac=ach / peak_tensor, traffic=None,
+                        peak_source=("MEASURED_PEAKS.json bf16_tflops_sustained (kernel timed inside a long step)" if peaks
+                                     else "NVIDIA H100 SXM data sheet, dense FP16/BF16 at 700 W (not a measured ceiling)"),
                         launch_ms=ki["pass1_ms"], algorithmic_flops_per_launch=ki["pass1_flops"],
                         issued_tensor_tflops=issued, frac_issued=issued / peak_tensor,
                         note=("achieved counts the ALGORITHMIC 2*n_q*n*d flops of the pairwise-distance sweep over the summed duration "
                               "of its launches (pilot wave + rest; rows the fp16 tier cannot certify are swept again in split "
                               "precision, n_resweep of them). The fp16 tier issues K = d+3 padded to 64 instead of 50, plus a 1/16 "
                               "sample of the candidate tiles for the starting threshold: issued_tensor_tflops / frac_issued say how "
-                              "busy the tensor pipe is. Each 256x128 score tile is 8 MMAs (512 tensor cycles) against one TMEM "
-                              "hand-off + 4 tcgen05.ld round trips per epilogue warp, so the sweep is paced by the accumulator "
-                              "hand-off, not by the MMAs (DESIGN.md section 5)"),
+                              "busy the tensor pipe is. Each 128x128 score tile is two warpgroups' wgmma.m64n128k16 k-steps; a "
+                              "warpgroup examines its scores in registers while the other one's MMAs run (DESIGN.md section 5)"),
                         n_resweep=ki.get("n_resweep", 0),
                         share_of_step=ki["pass1_ms"] / ms_step)
     else:
-        fp32_peak = 148 * 128 * 2 * sm_max * 1e6 / 1e12
+        import torch
+
+        sms = torch.cuda.get_device_properties(local_rank).multi_processor_count
+        fp32_peak = sms * 128 * 2 * sm_max * 1e6 / 1e12
         roofline = dict(bound="tensor", kernel="knn_pass1_kernel", achieved=ach, peak=peak_tensor, unit="TFLOP/s",
                         frac=ach / peak_tensor, traffic=None, launch_ms=ki["pass1_ms"], algorithmic_flops_per_launch=ki["pass1_flops"],
                         note=f"fp32 FFMA path (d too large for the tensor-core tiles); CUDA-core ceiling {fp32_peak:.1f} TFLOP/s",

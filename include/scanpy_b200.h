@@ -1,4 +1,4 @@
-/* scanpy_b200.h — C ABI of libscanpy_b200.so: the B200-native (sm_100a) kernels behind
+/* scanpy_b200.h — C ABI of libscanpy_b200.so: the H100-native (sm_90a) kernels behind
  * scanpy's  sc.pp.pca -> sc.pp.neighbors -> sc.tl.leiden  hot path.
  *
  * The reference (scverse/scanpy @ fabadb94) is pure Python and has no FFI of its own: its hot
@@ -71,8 +71,7 @@ typedef struct sb2_knn_info {
   float pass1_ms;           /* CUDA-event duration of all first-pass sweep launches on the ctx stream */
   double pass1_flops;       /* 2 * n_query * n_points * d: the algorithmic flops of that launch */
   double pass1_issued_flops; /* flops actually issued (tensor path: padded tiles x split-precision K axis) */
-  int32_t pass1_tensor;     /* 2 = knn_sweep2_kernel (tcgen05 N=256, default), 1 = knn_pass1_tc_kernel (first-generation tcgen05
-                               sweep: SB2_KNN_V=1 or K axes too wide for generation 2), 0 = knn_pass1_kernel (fp32 FFMA) */
+  int32_t pass1_tensor;     /* 2 = knn_sweep2_kernel (wgmma, default), 0 = knn_pass1_kernel (fp32 FFMA) */
   int64_t n_resweep;        /* rows the fp16 tier left uncertified, swept again in split precision (tensor path) */
 } sb2_knn_info;
 
@@ -160,7 +159,7 @@ int32_t sb2_pca_stream_project_f32(sb2_ctx* ctx, int64_t n_chunk, int32_t g, con
  * array (q0 % 128 == 0 unless n_query == n_points).  k includes the query itself: column 0 of
  * the outputs is the query row with distance 0 (src/scanpy/neighbors/_common.py:74-98).
  * Outputs [n_query x k]: d_idx int32 (global row ids), d_dist float64, ascending by (distance, id).
- * d <= 150, k <= 56.  Exactness: a fast first pass (tcgen05 fp16 / split-fp16 sweeps; SB2_KNN_PASS1=ffma selects the
+ * d <= 150, k <= 56.  Exactness: a fast first pass (wgmma fp16 / split-fp16 sweeps; SB2_KNN_PASS1=ffma selects the
  * fp32 CUDA-core sweep, k <= 30) proposes 32 (k <= 24) or 64 candidates per query, an fp64 re-score certifies the top-k
  * against a rounding-error bound, uncertified rows are recomputed exactly. */
 int32_t sb2_knn_l2_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, const float* d_x, int64_t q0, int64_t n_query,

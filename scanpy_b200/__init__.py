@@ -1,4 +1,4 @@
-"""scanpy_b200 — B200-native (sm_100a) `pp.pca -> pp.neighbors -> tl.leiden` with scanpy's signatures.
+"""scanpy_b200 — H100-native (sm_90a) `pp.pca -> pp.neighbors -> tl.leiden` with scanpy's signatures.
 
     import scanpy_b200 as sb
     sb.pp.pca(adata); sb.pp.neighbors(adata); sb.tl.leiden(adata)

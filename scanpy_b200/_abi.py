@@ -1,7 +1,7 @@
 """ctypes binding of libscanpy_b200.so (the C ABI declared in include/scanpy_b200.h).
 
 This is the only module that touches the shared library.  There is NO CPU path: if the
-library cannot be loaded, or no sm_100 device is present, every entry point raises.
+library cannot be loaded, or no sm_90 device is present, every entry point raises.
 torch is used here strictly as plumbing: device allocations (torch.empty(device='cuda')),
 host<->device copies and the current CUDA stream handle; all arithmetic happens in the .so.
 """
@@ -125,7 +125,7 @@ _lib = None
 
 
 def build(force: bool = False) -> Path:
-    """Compile the CUDA sources for sm_100a into scanpy_b200/libscanpy_b200.so (in-tree)."""
+    """Compile the CUDA sources for sm_90a into scanpy_b200/libscanpy_b200.so (in-tree)."""
     srcs = list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cuh")) + [_PKG.parent / "include" / "scanpy_b200.h"]
     newest = max(p.stat().st_mtime for p in srcs)
     if force or not LIB_PATH.exists() or LIB_PATH.stat().st_mtime < newest:

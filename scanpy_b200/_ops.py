@@ -137,9 +137,8 @@ def _pca_csr_overlapped(ctx, x, n_comps: int, seed: int, n_chunks: int = 8):
     in `n_chunks` row ranges on a side stream, and as each range lands the compute stream adds its column statistics and
     Gram matrix (sb2_pca_stream_accumulate_f32 - the out-of-core entry point, pointed at the resident arrays).  The
     projection then runs over the whole resident matrix.  Same arithmetic as solver 1 up to the fp64 summation order.
-    OPT-IN (SB2_PCA_OVERLAP=1): measured on B200 at 1.3M x 2000 from page-locked arrays, pca() takes 78 ms of wall time
-    this way against 62 ms of device work, but the bench's e2e did not improve (0.489 s vs 0.471 s without it, within
-    box-to-box noise) - the 21 ms upload is already a small part of the step - so the plain upload stays the default."""
+    OPT-IN (SB2_PCA_OVERLAP=1): at the bench workload the upload is a small part of the step, so the plain upload stays
+    the default."""
     torch = _torch()
     n, g = x.shape
     nnz = int(x.nnz)

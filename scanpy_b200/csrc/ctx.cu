@@ -31,8 +31,8 @@ int32_t sb2_ctx_create(int32_t device, void* stream, uint32_t flags, sb2_ctx** o
   sb2_ctx* c = new sb2_ctx();
   c->device = device;
   SB2_CUDA(cudaGetDeviceProperties(&c->prop, device));
-  if (c->prop.major != 10) {
-    sb2_set_error("device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, c->prop.major,
+  if (c->prop.major != 9 || c->prop.minor != 0) {
+    sb2_set_error("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, c->prop.major,
                   c->prop.minor);
     delete c;
     return SB2_E_UNSUPPORTED;

@@ -1,4 +1,4 @@
-// graph.cu — UMAP fuzzy simplicial set -> symmetric connectivities CSR (sm_100a).
+// graph.cu — UMAP fuzzy simplicial set -> symmetric connectivities CSR (sm_90a).
 //
 // Replaces umap.umap_.fuzzy_simplicial_set(...).tocsr() as called by the reference at
 // src/scanpy/neighbors/_connectivity.py:124-138 (arithmetic spec: SURVEY.md Appendix A2;

@@ -1,4 +1,4 @@
-// knn.cu — exact brute-force euclidean kNN on the n x d float32 embedding (sm_100a).
+// knn.cu — exact brute-force euclidean kNN on the n x d float32 embedding (sm_90a).
 //
 // Replaces sklearn's KNeighborsTransformer(algorithm='brute') as built by the reference at
 // src/scanpy/neighbors/__init__.py:754-768 (ArgKmin: GEMM-shaped middle term with fp64
@@ -534,26 +534,8 @@ int32_t read_count(sb2_ctx* ctx, const unsigned long long* d_cnt, int64_t* out) 
   return SB2_OK;
 }
 
-// ---- the two generations of the tensor-core sweep behind one interface (tensor_tiers below) ----
-struct SweepV1 {   // knn_tc.cu: 256-query CTAs x 128-candidate tiles, one 32/64-proposal list per row (SB2_KNN_V=1)
-  KnnTcShape sh;
-  bool shape(const sb2_ctx* ctx, int d, int terms) { return knn_tc_shape(ctx, d, terms, &sh); }
-  static int list_m(int k, bool force64) { return (k > 24 || force64) ? 64 : 32; }
-  static int sub(int list_m) { return list_m; }
-  int wave_rows(const sb2_ctx* ctx) const { return ctx->prop.multiProcessorCount * sh.qh * TILE; }
-  size_t a_halves(int64_t n) const { return knn_tc_image_halves(sh, n); }
-  size_t b_halves(int64_t n) const { return knn_tc_image_halves(sh, n); }
-  int32_t build(sb2_ctx* ctx, const float* x, int64_t n, int d, const unsigned int* mn, const int32_t* g, int64_t gb, __half* A,
-                __half* B, float* inv_s2, float* dnorm, unsigned int* dmax) const {
-    return knn_tc_build_images(ctx, sh, x, n, d, mn, g, gb, A, B, inv_s2, dnorm, dmax);
-  }
-  int32_t sweep(sb2_ctx* ctx, const __half* A, int64_t a_tile0, const __half* B, int64_t n_points, int64_t n_query, int lm,
-                float* cs, int32_t* ci, double* fl, bool est) const {
-    return knn_tc_sweep(ctx, sh, A, a_tile0, B, n_points, n_query, lm, cs, ci, fl, est);
-  }
-  void coefs(double* cq, double* cn) const { knn_tc_error_coefs(sh, cq, cn); }
-};
-struct SweepV2 {   // knn_tc2.cu: 128-query CTAs x 256-candidate tiles (UMMA N = 256), four sub-lists per row (default)
+// ---- the tensor-core sweep of knn_tc2.cu behind the interface tensor_tiers uses ----
+struct SweepV2 {   // knn_tc2.cu: 128-query CTAs x 128-candidate tiles (wgmma N = 128), four sub-lists per row
   KnnTc2Shape sh;
   bool shape(const sb2_ctx* ctx, int d, int terms) { return knn_tc2_shape(ctx, d, terms, terms == 1, &sh); }
   static int list_m(int k, bool force_big) { return (k > 24 || force_big) ? 128 : 64; }
@@ -698,7 +680,7 @@ int32_t tensor_tiers(TierState& t, bool split_only, bool force_big_list) {
 
 // Exact kNN: a fast first pass proposes candidates per query, an fp64 re-score certifies the top-k against a rigorous
 // rounding-error bound, rows without a certificate are recomputed exactly.  First pass: the tensor-core tiers above
-// (default: knn_tc2.cu; SB2_KNN_V=1: the first-generation kernel of knn_tc.cu) or the fp32 CUDA-core sweep (SB2_KNN_PASS1=ffma).
+// (knn_tc2.cu) or the fp32 CUDA-core sweep (SB2_KNN_PASS1=ffma).
 extern "C" int32_t sb2_knn_l2_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, const float* d_x, int64_t q0,
                                   int64_t n_query, int32_t k, int32_t* d_idx, double* d_dist, sb2_knn_info* info) {
   SB2_CHECK_ARG(ctx && d_x && d_idx && d_dist, "null pointer");
@@ -722,9 +704,7 @@ extern "C" int32_t sb2_knn_l2_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, con
   SB2_TRY(scr.alloc(&maxnorm, 4));
   const char* force = getenv("SB2_KNN_PASS1");
   const char* tiers = getenv("SB2_KNN_TIERS");
-  const char* gen = getenv("SB2_KNN_V");
-  const bool use_tc = knn_tc_supported(d) && !(force && strcmp(force, "ffma") == 0);
-  const bool use_v1 = gen && strcmp(gen, "1") == 0;
+  const bool use_tc = knn_tc2_supported(d) && !(force && strcmp(force, "ffma") == 0);
   const bool split_only = tiers && strcmp(tiers, "3") == 0;
   const char* list_env = getenv("SB2_KNN_LIST");
   const bool big_list = list_env && (strcmp(list_env, "64") == 0 || strcmp(list_env, "128") == 0);
@@ -749,8 +729,7 @@ extern "C" int32_t sb2_knn_l2_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, con
   int64_t n_resweep = 0;
   if (use_tc) {
     TierState t{ctx, &scr, d_x, n_points, q0, n_query, d, k, maxnorm, wq1, wq2, wub1, wub2, wcnt, d_idx, d_dist, &evs};
-    if (use_v1) SB2_TRY(tensor_tiers<SweepV1>(t, split_only, big_list));
-    else SB2_TRY(tensor_tiers<SweepV2>(t, split_only, big_list));
+    SB2_TRY(tensor_tiers<SweepV2>(t, split_only, big_list));
     issued_flops = t.issued_flops;
     n_resweep = t.n_resweep;
   } else {
@@ -798,13 +777,13 @@ extern "C" int32_t sb2_knn_l2_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, con
     info->pass1_ms = evs.total_ms();
     info->pass1_flops = 2.0 * (double)n_query * (double)n_points * (double)d;
     info->pass1_issued_flops = issued_flops;
-    info->pass1_tensor = use_tc ? (use_v1 ? 1 : 2) : 0;
+    info->pass1_tensor = use_tc ? 2 : 0;
     info->n_resweep = n_resweep;
   }
   return SB2_OK;
 }
 
-// Debug / test entry: the raw proposals of ONE cold-start tensor sweep (generation 2) in the chosen operand format, with
+// Debug / test entry: the raw proposals of ONE cold-start tensor sweep in the chosen operand format, with
 // everything the rounding-error certificate is computed from, so that a test can MEASURE |s_tensor - s_exact| on the
 // hardware against the bound knn_rescore_kernel uses (tests/test_gpu_parity.py::test_knn_tensor_score_error_within_bound).
 //   d_score / d_idx [n_points x list_m]: proposal scores in the kernel's scaled units and their point ids (-1: unused)

@@ -1,49 +1,23 @@
-// knn_internal.cuh — interface between knn.cu (host entry, re-score, fallback) and knn_tc.cu (tensor-core sweeps)
+// knn_internal.cuh — interface between knn.cu (host entry, re-score, fallback) and knn_tc2.cu (tensor-core sweep)
 #pragma once
 #include <cuda_fp16.h>
 
 #include "common.cuh"
 
-// tile shape of one tensor-core sweep: `terms` = 1 (fp16 operands, fast first tier) or 3 (split precision, 22 bits)
-struct KnnTcShape {
-  int qh;       // 128-query tiles per CTA (2 or 1)
-  int nsplit;   // slices the K axis of a candidate image is staged in (1, 2, 4)
-  int nstage;   // depth of the candidate ring
-  int kpad;     // padded K axis (terms*d + 3 rounded up to 16*nsplit)
-  int terms;
-  size_t smem;
-};
-bool knn_tc_supported(int d);
-bool knn_tc_shape(const sb2_ctx* ctx, int d, int terms, KnnTcShape* out);
-size_t knn_tc_image_halves(const KnnTcShape& sh, int64_t n_rows);
-// operand images for rows [0, n_rows) of X (or, with d_gather, rows gather_base + d_gather[i]); Aimg or Bimg may be
-// null; d_dnorm[i] / *d_dmax_bits (optional) receive |x_i - fp16(x_i)| and its maximum; d_inv_s2 receives 1/s^2 of the power-of-two scale the scores carry (score_true = score * inv_s2)
-int32_t knn_tc_build_images(sb2_ctx* ctx, const KnnTcShape& sh, const float* d_x, int64_t n_rows, int d,
-                            const unsigned int* d_maxnorm_bits, const int32_t* d_gather, int64_t gather_base,
-                            __half* Aimg, __half* Bimg, float* d_inv_s2, float* d_dnorm = nullptr,
-                            unsigned int* d_dmax_bits = nullptr);
-// proposals (unsorted, list_m per query; unused slots: score -inf, id -1) for the n_query rows whose A images
-// start at tile a_tile0; *issued_flops is incremented; estimate = false starts the lists cold (no sampled threshold:
-// every row ends with its true top list_m, the certificate can only fail on exact ties)
-int32_t knn_tc_sweep(sb2_ctx* ctx, const KnnTcShape& sh, const __half* Aimg, int64_t a_tile0, const __half* Bimg,
-                     int64_t n_points, int64_t n_query, int list_m, float* cand_score, int32_t* cand_idx, double* issued_flops,
-                     bool estimate = true);
-void knn_tc_error_coefs(const KnnTcShape& sh, double* c_q, double* c_n);
-
-// ---- second-generation sweep (knn_tc2.cu): 128-query CTAs x 256-candidate tiles (UMMA N = 256), 16 epilogue warps,
-// four register-resident sub-lists per query row (one per 64-column quarter of a tile) ----
+// ---- tensor-core sweep (knn_tc2.cu): 128-query CTAs x 128-candidate tiles (wgmma N = 128), two consumer warpgroups,
+// four register-resident sub-lists per query row (one per column class of the accumulator fragment) ----
 struct KnnTc2Shape {
   int nsplit;   // slices the K axis of a candidate image is staged in (1, 2, 4, 8)
   int nstage;   // depth of the candidate ring
   int kpad;     // padded K axis (terms*d + 3 rounded up to 16*nsplit)
   int terms;
-  int est;      // 1: shared memory holds the exchange area of the sampled starting threshold
+  int est;      // 1: the sweep may start from a sampled threshold
   size_t smem;
 };
 bool knn_tc2_supported(int d);
 bool knn_tc2_shape(const sb2_ctx* ctx, int d, int terms, bool want_estimate, KnnTc2Shape* out);
 size_t knn_tc2_a_halves(const KnnTc2Shape& sh, int64_t n_rows);   // query images: tiles of 128 rows
-size_t knn_tc2_b_halves(const KnnTc2Shape& sh, int64_t n_rows);   // candidate images: tiles of 256 rows
+size_t knn_tc2_b_halves(const KnnTc2Shape& sh, int64_t n_rows);   // candidate images: tiles of 128 rows
 int32_t knn_tc2_build_images(sb2_ctx* ctx, const KnnTc2Shape& sh, const float* d_x, int64_t n_rows, int d,
                              const unsigned int* d_maxnorm_bits, const int32_t* d_gather, int64_t gather_base,
                              __half* Aimg, __half* Bimg, float* d_inv_s2, float* d_dnorm = nullptr,

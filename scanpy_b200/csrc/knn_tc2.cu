@@ -1,45 +1,31 @@
-// knn_tc2.cu — tensor-core sweep of the exact kNN, second generation (sm_100a: tcgen05.mma N = 256 + TMEM + bulk-copy ring).
+// knn_tc2.cu — tensor-core sweep of the exact kNN (sm_90a: wgmma m64n128k16 from shared memory + bulk-copy ring).
 //
-// Same contract as the first-generation sweep (knn_tc.cu): per query keep the proposals whose score
+// Per query keep the proposals whose score
 //     s(q,c) = q.c - |c|^2/2        (d^2 = |q|^2 - 2 s)
 // is largest, plus a rigorous bound on the rounding error of s, so that knn_rescore_kernel can certify the exact fp64
-// top-k.  Operand formats (terms = 1: fp16, K = d+3; terms = 3: split fp16, K = 3d+3) are unchanged.
+// top-k.  Operand formats (coordinates scaled by a power of two so that max|x| is in [100, 200)):
+//   terms = 1  fp16 operands            A = [q_hi | 1 1 1],               B = [c_hi | h0 h1 h2]              K = d+3
+//   terms = 3  split fp16 (22 bits)     A = [q_hi | q_hi | q_lo | 1 1 1], B = [c_hi | c_lo | c_hi | h0 h1 h2]  K = 3d+3
+// with hi = fp16(x), lo = fp16(x - hi) and h0+h1+h2 = -|c|^2/2 (three-way fp16 split); K is padded to a multiple of 16
+// (d = 50: 64 and 160).  knn.cu runs terms = 1 first and re-sweeps the rows it cannot certify with terms = 3.
 //
-// What round 2 measured on the first generation (profiles/README.md, scripts/ubench/mma_smem_contention.cu,
-// alu_max_rate.cu, the SB2_KNN_DBG / SB2_KNN2_NOSCAN cycle stamps):
-//   * a 128x128x16 tcgen05.mma with both operands in shared memory reads 8 KB per 64 tensor cycles = 128 B/clk, ALL of
-//     the shared-memory bandwidth; next to the bulk-copy ring the pipe delivered one MMA per ~105 cycles (850 cycles per
-//     256x128 tile even with an EMPTY epilogue, 512 ideal).  128x256x16 MMAs (12 KB per 128 cycles) hold 131-138 cycles
-//     under the same traffic: with N = 256 and scanners that only load and release, this kernel runs at 521-546 cycles
-//     per 128x256 tile (tensor floor 512; power-capped at ~1000 W: 1450-1630 TFLOP/s issued);
-//   * the first generation's epilogue (two warps per scheduler, one dependent max tree each) had too little instruction
-//     level parallelism: ~1200 cycles per tile.
-// Hence this shape (one CTA per SM, 18 warps):
-//   CTA = 128 queries (UMMA M) x all candidate tiles of 256 points (UMMA N = 256), two 256-column accumulator buffers.
-//     warps 0-15  epilogue, FOUR warps per TMEM lane quadrant: warp (quadrant q, column quarter cq) owns rows
-//                 32q..32q+31 x columns 64cq..64cq+63 of every tile: tcgen05.ld.32x32b.x32 of its first chunk, examine,
-//                 load the second, release the buffer (16th arrival), examine.  Each (row, column quarter) keeps its
-//                 OWN register-resident proposal sub-list (16 or 32 scores in groups of 8 with group minima; ids
-//                 write-only to global memory): no cross-warp traffic in the loop.  A point outside all four sub-lists
-//                 of a row scored at most max(tau_0..tau_3), which is what the re-score certificate uses.
-//     warp 16     producer: 1-D cp.async.bulk of pre-arranged candidate images (or K-slices of them) into an mbarrier
-//                 ring that takes all the shared memory left
-//     warp 17     MMA issuer (whole-warp loop, elect.sync inside the asm block, operands on the uniform datapath);
-//                 tcgen05.commit frees the ring stage and publishes the accumulator buffer; owns TMEM alloc/dealloc
-//   Service warps carry the highest warp ids (the sub-partition arbiter prefers them among eligible warps).
+// Shape (one CTA per SM, 9 warps):
+//   CTA = 128 queries x all candidate tiles of 128 points.
+//     warps 0-7   two consumer warpgroups; warpgroup g owns query rows 64g..64g+63 and issues, per tile, the k-steps of
+//                 wgmma.m64n128k16 (A = its 64 query rows, B = the staged candidate tile, both from shared memory, fp32
+//                 accumulators in registers), waits for them, hands the ring stage back and examines the 64 x 128
+//                 scores in registers.  While one warpgroup examines, the other one's MMAs run.  In the accumulator
+//                 fragment a thread holds two rows and, of each, the 32 columns with (column / 2) % 4 = lane % 4; every
+//                 (row, lane % 4) keeps its OWN register-resident proposal sub-list (16 or 32 scores in groups of 8 with
+//                 group minima; ids write-only to global memory): four disjoint sub-lists per row, no cross-thread
+//                 traffic in the loop.  A point outside all four sub-lists of a row scored at most max(tau_0..tau_3),
+//                 which is what the re-score certificate uses.
+//     warp 8      producer: 1-D cp.async.bulk of pre-arranged candidate images (or K-slices of them) into an mbarrier
+//                 ring that takes the shared memory left after the query image
 //   Starting threshold: the first n/16 visits sweep every 16th tile and keep the 6 largest chunk maxima per (row,
-//   quarter); the four quarters of a row are merged through shared memory once (named barrier over the 16 epilogue
-//   warps) and the 6th largest of the 24 seeds all four sub-lists (rank ~96 of the row, as before).
+//   sub-list); the four sub-lists of a row (four lanes of one warp) are merged by shuffles once and the 6th largest of
+//   the 24 seeds all four (rank ~96 of the row).
 //   Sweep front: CTAs walk the candidate tiles cyclically, starting where the running CTAs currently are (g_knn2_front).
-// Where the time goes now (1.3M x 50, k = 15): 1000-1100 cycles per tile against the 512 of the tensor pipe.  The
-// examine phases cost each warp ~600 cycles per tile (~290 of them the ALU pipe's floor for the max trees: FMNMX3 issues
-// every 2 cycles per scheduler, FMNMX every cycle), and ~6 % of the chunk scans take the insertion path (~150 dependent
-// instructions for one lane); since the release of an accumulator buffer needs all 16 warps, whichever warp is inserting
-// gates the hand-off of nearly every tile.  Two decouplings were built, measured and dropped (git history, DESIGN.md):
-//   - scanners that push (row, id, score) into a shared-memory queue drained by inserter warps holding one list per row:
-//     exact, but the claim / release-acquire traffic cost more than it saved (1330 cycles per tile);
-//   - both chunks loaded before anything is examined and the sub-lists kept in shared memory (early release): the
-//     insertion walk over shared memory and the 96-register cap (18 warps) made each examine phase slower (1180-1240).
 #include <cuda_fp16.h>
 #include <float.h>
 
@@ -50,23 +36,18 @@
 namespace {
 using namespace tcptx;
 
-constexpr int QM = 128;            // queries per CTA (UMMA M, TMEM lanes)
-constexpr int CN = 256;            // candidates per tile (UMMA N, TMEM columns per accumulator buffer)
+constexpr int QM = 128;            // queries per CTA (two warpgroups of M = 64)
+constexpr int CN = 128;            // candidates per tile (wgmma N)
 constexpr int MAXST = 8;           // upper bound of the ring depth
-constexpr int BAR_BYTES = 1024;    // mbarriers + TMEM slot IN FRONT of the operand images (fixed addresses)
-constexpr int NEPI = 16;           // epilogue warps
-constexpr int NQUART = 4;          // column quarters (epilogue warps per TMEM lane quadrant)
-constexpr int THREADS = (2 + NEPI) * 32;
-// Service warps carry the HIGHEST warp ids: the sub-partition arbiter prefers the highest warp id among eligible warps
-// (B300_MICROARCH: "highest-wid-first"), so the producer and the MMA issuer are never starved by the four epilogue
-// warps they share a scheduler with.
-constexpr int W_PROD = NEPI, W_MMA = NEPI + 1;
+constexpr int BAR_BYTES = 1024;    // mbarriers IN FRONT of the operand images
+constexpr int NCONS = 8;           // consumer warps (two warpgroups)
+constexpr int THREADS = (NCONS + 1) * 32;
+constexpr int W_PROD = NCONS;
+constexpr int NSUB = 4;            // sub-lists per query row
 constexpr int EST_R = 6;
-constexpr int EST_BYTES = QM * NQUART * EST_R * 4;   // exchange area of the threshold estimate
-constexpr uint32_t SBO = 128;                  // bytes between 8-row groups (core matrices contiguous)
-constexpr uint32_t LBO_A = QM * 16;            // bytes between K-chunks of a 128-row image  [kc][row-group][8][8]
-constexpr uint32_t LBO_B = CN * 16;            // ... of a 256-row image
-constexpr uint32_t IDESC = umma_idesc_f16_m128(CN);
+constexpr uint32_t SBO = 128;              // bytes between 8-row groups (core matrices contiguous)
+constexpr uint32_t LBO = QM * 16;          // bytes between K-chunks of a 128-row image  [kc][row-group][8][8]
+static_assert(QM == CN, "query and candidate images share one layout");
 
 // scale: power of two s with s*R in [100, 200]  ->  fp16 range is safe for coordinates and for s^2 R^2/2
 __device__ __forceinline__ float tc_scale_from_maxnorm(unsigned int maxnorm_bits) {
@@ -77,8 +58,8 @@ __device__ __forceinline__ float tc_scale_from_maxnorm(unsigned int maxnorm_bits
   return exp2f((float)e);
 }
 
-// X[n,d] -> operand images of `tile_rows` points each (128: query images, 256: candidate images), stored exactly as
-// the UMMA "no-swizzle, K-major" shared-memory layout wants them (8x8 fp16 core matrices, K-chunk-major), so a tile
+// X[n,d] -> operand images of `tile_rows` points each (128 for query and candidate images), stored exactly as the
+// wgmma "no-swizzle, K-major" shared-memory layout wants them (8x8 fp16 core matrices, K-chunk-major), so a tile
 // (or a K-slice of it) is staged by ONE 1-D bulk copy.
 //   is_a = 1: A = [hi | hi | lo | 1 1 1]  (terms = 3)   or  [hi | 1 1 1]      (terms = 1)
 //   is_a = 0: B = [hi | lo | hi | h0 h1 h2]             or  [hi | h0 h1 h2]   with h0+h1+h2 = -|x|^2 s^2 / 2
@@ -93,7 +74,7 @@ knn_tc2_prep_kernel(const float* __restrict__ X, int64_t n, int d, int kpad, int
   const int64_t t = blockIdx.x;
   const float s = tc_scale_from_maxnorm(*maxnorm_bits);
   if (t == 0 && threadIdx.x == 0 && inv_s2) *inv_s2 = 1.0f / (s * s);
-  __shared__ __half hn3[CN][3];
+  __shared__ __half hn3[256][3];
   const int kd = terms * d;  // coordinates on the K axis before the three norm slots
   if ((int)threadIdx.x < tile_rows) {
     const int64_t p = t * tile_rows + threadIdx.x;
@@ -192,18 +173,15 @@ __device__ __forceinline__ void list_insert(SubList<NG>& L, int32_t* __restrict_
   for (int g = 1; g < NG; ++g) t = fminf(t, L.gm[g]);
   L.tau = t;
 }
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+__device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 __device__ __forceinline__ float max8u(const uint32_t* v) {
   return fmax3(fmax3(__uint_as_float(v[0]), __uint_as_float(v[1]), __uint_as_float(v[2])),
                fmax3(__uint_as_float(v[3]), __uint_as_float(v[4]), __uint_as_float(v[5])),
                fmaxf(__uint_as_float(v[6]), __uint_as_float(v[7])));
 }
-// examine one 32-column chunk of the row (values already in registers).  Fast path: a two-level 3-input max tree (four
-// independent quarter maxima, so the FMNMX3 latencies overlap) and one compare.  Rare path: visit the quarters whose
+// examine one 32-value chunk of the row (values already in registers; value m is candidate cand0 + 8 (m / 2) + m % 2,
+// the columns one thread holds in the wgmma accumulator fragment).  Fast path: a max tree (four independent quarter
+// maxima, so the latencies overlap) and one compare.  Rare path: visit the quarters whose
 // maximum beats tau, copy the quarter's eight values aside and pull its maxima out one by one.  The quarter loop is
 // NOT unrolled: one copy of the extraction and insertion code per call site keeps the kernel in the instruction caches.
 template <int NG>
@@ -229,7 +207,8 @@ __device__ __forceinline__ void scan_chunk(SubList<NG>& L, int32_t* __restrict__
             w[jj] = hset ? 0xff800000u : w[jj];  // knock the maximum out (-inf)
             found |= hset;
           }
-          const int32_t cand = cand0 + q * 8 + j;
+          const int m = q * 8 + j;                          // value m of the chunk is column 8 (m / 2) + m % 2
+          const int32_t cand = cand0 + ((m >> 1) << 3) + (m & 1);
           if (cand < n_points) list_insert(L, id, hq, cand);
           hq = max8u(w);
         } while (hq > L.tau);
@@ -252,57 +231,35 @@ __device__ __forceinline__ void est_chunk(float (&est)[LEN], const uint32_t (&v)
   est_push(est, fmaxf(fmax3(max8u(&v[0]), max8u(&v[8]), max8u(&v[16])), max8u(&v[24])));
 }
 
-// nks = k-steps (16 columns of the K axis) per staged slice, nsplit = slices per candidate image.  Everything the MMA
-// warp derives its operands from is a kernel parameter combined by add / multiply only (a division would move the
-// values to the vector datapath and every tcgen05.mma would need its operands copied back through R2UR).
-// NOSCAN (timing experiments only, SB2_KNN2_NOSCAN=1): the epilogue loads and releases but does not examine.
-// SB2_KNN2_STAMP=1: CTA 0, warp 2 records clock64 / globaltimer around its visit loop (cycles per visit and the SM clock
-// actually delivered under this kernel's load); read back by knn_tc2_sweep and printed to stderr
+// nks = k-steps (16 columns of the K axis) per staged slice, nsplit = slices per candidate image.
 // Sweep front: CTAs walk the candidate tiles cyclically, each starting where the CTAs already running currently are
 // (the order of the candidates is irrelevant to the result).  All resident CTAs then stream the same few tiles at the
 // same time and the candidate images (166 MB at 1.3M x 50, more than the L2) are read from HBM about once per wave of
 // CTAs instead of once per CTA.  "Where the running CTAs are" is the MEAN position of the pack, (sweep visits so far) /
-// (resident CTAs): the first version started a new CTA at the position last published by ANY running CTA, so the
-// spread of the pack was inherited and widened from wave to wave (a random walk over 68 waves: ncu showed 114 GB of
-// DRAM reads per launch, L2 hit rate 77 %, profiles/r2_ncu_metrics_knn_sweep2.txt); re-centring every new CTA on the
-// mean bounds the spread by the drift of a single lap.
+// (resident CTAs): starting a new CTA at the position last published by ANY running CTA lets the spread of the pack
+// grow from wave to wave; re-centring every new CTA on the mean bounds it by the drift of a single lap.
 __device__ unsigned long long g_knn2_front;   // sweep-proper visits of all CTAs of this launch, in units of 16 tiles
-__device__ unsigned long long g_knn2_stamp[4];
-__device__ unsigned long long g_knn2_phase[2][8];
-__device__ __forceinline__ unsigned long long gtimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
-}
-template <int NG, int MODE>
+template <int NG>
 __global__ void __launch_bounds__(THREADS, 1)
 knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bimg, int nks, int nsplit, int nstage,
-                  uint32_t mma_part16, uint32_t mma_atile16, int mma_visits, int64_t n_btiles, int64_t n_est,
-                  int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points, float* __restrict__ cand_score,
-                  int32_t* __restrict__ cand_idx) {
+                  int64_t n_btiles, int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points,
+                  float* __restrict__ cand_score, int32_t* __restrict__ cand_idx) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t part_b = (uint32_t)(CN * 16 * 2) * (uint32_t)nks;      // bytes per staged K-slice of a candidate image
-  const uint32_t tile_b = part_b * (uint32_t)nsplit;                    // bytes per 256-row candidate image
-  const uint32_t tile_a = tile_b >> 1;                                  // bytes per 128-row query image
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);   // fixed offset: barrier addresses stay uniform values
+  const uint32_t tile_b = part_b * (uint32_t)nsplit;                    // bytes per 128-row image (query or candidate)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
   unsigned char* As = smem_raw + BAR_BYTES;
-  unsigned char* Bs0 = As + tile_a;
-  uint64_t* full = bars;                  // [MAXST] producer -> MMA
-  uint64_t* empty = bars + MAXST;         // [MAXST] MMA (commit) -> producer
+  unsigned char* Bs0 = As + tile_b;
+  uint64_t* full = bars;                  // [MAXST] producer -> consumers
+  uint64_t* empty = bars + MAXST;         // [MAXST] consumer warps -> producer
   uint64_t* afull = bars + 2 * MAXST;     // [1]
-  uint64_t* tfull = bars + 2 * MAXST + 1;    // [2] MMA (commit) -> epilogue
-  uint64_t* tempty = bars + 2 * MAXST + 3;   // [2] epilogue (16 warps) -> MMA
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAXST + 5);
-  int32_t* start_tile = reinterpret_cast<int32_t*>(bars + 2 * MAXST + 6);
-  static_assert((2 * MAXST + 6) * 8 + 4 <= BAR_BYTES, "barrier block");
-  float* est_x = reinterpret_cast<float*>(Bs0 + (size_t)nstage * part_b);  // [QM][NQUART][EST_R], present iff n_est > 0
+  int32_t* start_tile = reinterpret_cast<int32_t*>(bars + 2 * MAXST + 1);
+  static_assert((2 * MAXST + 2) * 8 <= BAR_BYTES, "barrier block");
 
-  // warp index through a shuffle: tells the compiler it is warp-uniform, so each role's branch is a converged region
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
-    for (int s = 0; s < nstage; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+    for (int s = 0; s < nstage; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NCONS); }
     mbar_init(afull, 1);
-    for (int b = 0; b < 2; ++b) { mbar_init(&tfull[b], 1); mbar_init(&tempty[b], NEPI); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     const unsigned long long f = *reinterpret_cast<volatile unsigned long long*>(&g_knn2_front);
     unsigned int nsm;
@@ -311,21 +268,13 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
     // mean tile of the pack now, plus the n_est visits this CTA spends on its threshold estimate before it joins
     *start_tile = (int32_t)((f * 16ull / resident + (unsigned long long)n_est) % (unsigned long long)n_btiles);
   }
-  if (warp == W_MMA) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (tmem_base != 0) __trap();  // a 512-column allocation can only start at lane 0, column 0 (the MMA warp relies on it)
 
   if (warp == W_PROD) {
     // ---------------- producer ----------------
     if (lane == 0) {
-      mbar_expect_tx(afull, tile_a);
-      bulk_g2s(As, reinterpret_cast<const unsigned char*>(Aimg) + (size_t)(qtile0 + (int64_t)blockIdx.x) * tile_a, tile_a, afull);
+      mbar_expect_tx(afull, tile_b);
+      bulk_g2s(As, reinterpret_cast<const unsigned char*>(Aimg) + (size_t)(qtile0 + (int64_t)blockIdx.x) * tile_b, tile_b, afull);
       // visit order: n_est sample tiles (every est_stride-th) for the threshold estimate, then every tile
       int s = 0;
       uint32_t use_phase = 1;  // parity of the previous use of stage s (first lap: nothing to wait for)
@@ -343,165 +292,117 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
         }
       }
     }
-  } else if (warp == W_MMA) {
-    // ---------------- MMA issuer (whole warp, elected thread issues) ----------------
-    mbar_wait(afull, 0);
-    // descriptor halves: lo = start address >> 4 | LBO field (bits 16..29); hi = SBO field | version; one k-step (two
-    // 8-column K-chunks) advances the start address by 2*LBO bytes
-    const uint64_t da0 = umma_desc(0, LBO_A, SBO), db0 = umma_desc(0, LBO_B, SBO);
-    const uint32_t desc_hi = (uint32_t)(da0 >> 32);  // identical for A and B (same SBO)
-    const uint32_t as16 = ((smem_u32(smem_raw) + BAR_BYTES) & 0x3FFFFu) >> 4;
-    const uint32_t a_lo0 = (uint32_t)da0 | as16;
-    const uint32_t b_lo0 = ((uint32_t)db0 | as16) + mma_atile16;   // Bs0 = As + one query image
-    constexpr uint32_t KSTEP_A16 = (2u * LBO_A) >> 4, KSTEP_B16 = (2u * LBO_B) >> 4;
-    int s = 0;
-    uint32_t ring_phase = 0;
-    // mma_part16 / mma_atile16 / mma_visits repeat part_b >> 4, tile_a >> 4 and n_est + n_btiles as parameters of their
-    // own, so that this warp's copies stay on the uniform datapath (the other warps use the vector ones)
-    constexpr bool PHASES_M = MODE == 2;
-    long long mph[3] = {0, 0, 0}, mtp = 0;
-    if (PHASES_M) mtp = clock64();
-#define SB2_MPH(i) if (PHASES_M) { const long long tn = clock64(); mph[i] += tn - mtp; mtp = tn; }
-    for (int c = 0; c < mma_visits; ++c) {
-      const int b = c & 1;
-      const int useb = c >> 1;
-      for (int p = 0; p < nsplit; ++p) {
-        mbar_wait(&full[s], ring_phase);
-        SB2_MPH(0)
-        if (p == 0 && useb > 0) mbar_wait(&tempty[b], (uint32_t)((useb - 1) & 1));
-        SB2_MPH(1)
-        tc_fence_after();
-        const uint32_t tm = (uint32_t)(b * CN);  // the CTA owns all 512 TMEM columns: allocation starts at column 0
-        uint32_t da = a_lo0 + (uint32_t)(p * nks) * KSTEP_A16;
-        uint32_t db = b_lo0 + (uint32_t)s * mma_part16;
-        if (p == 0) umma_f16_elect<false>(tm, da, db, desc_hi, IDESC); else umma_f16_elect<true>(tm, da, db, desc_hi, IDESC);
-#pragma unroll 4
-        for (int j = 1; j < nks; ++j) {
-          da += KSTEP_A16;
-          db += KSTEP_B16;
-          umma_f16_elect<true>(tm, da, db, desc_hi, IDESC);
-        }
-        tc_commit_elect(&empty[s]);   // ring stage reusable once these MMAs have read it
-        if (++s == nstage) { s = 0; ring_phase ^= 1u; }
-      }
-      tc_commit_elect(&tfull[b]);     // accumulator buffer b complete
-      SB2_MPH(2)
+    return;
+  }
+
+  // ---------------- consumers: thread <-> (two query rows, sub-list lane % 4) ----------------
+  const int g = warp >> 2;                                   // warpgroup: query rows 64g .. 64g+63
+  const int sl = lane & 3;                                   // sub-list = column class of the fragment
+  const int row0 = 64 * g + 16 * (warp & 3) + (lane >> 2);   // rows row0 and row0 + 8
+  const int64_t ql0 = (int64_t)blockIdx.x * QM + row0, ql1 = ql0 + 8;
+  const bool valid0 = ql0 < n_query, valid1 = ql1 < n_query;
+  constexpr int LS = 8 * NG, LM = NSUB * LS;
+  float* sc0 = cand_score + (valid0 ? ql0 : 0) * LM + sl * LS;
+  float* sc1 = cand_score + (valid1 ? ql1 : 0) * LM + sl * LS;
+  int32_t* id0 = cand_idx + (valid0 ? ql0 : 0) * LM + sl * LS;
+  int32_t* id1 = cand_idx + (valid1 ? ql1 : 0) * LM + sl * LS;
+  SubList<NG> L0, L1;
+  L0.tau = INFINITY;
+  L1.tau = INFINITY;
+#pragma unroll
+  for (int i = 0; i < LS; ++i) {
+    if (valid0) id0[i] = -1;
+    if (valid1) id1[i] = -1;
+  }
+  // During the estimate phase the EST_R running chunk maxima live in L.ls[0..EST_R) (the sub-list proper does not exist
+  // yet): one register array serves both phases.
+  static_assert(EST_R <= LS, "estimate aliases the list registers");
+#pragma unroll
+  for (int i = 0; i < LS; ++i) { L0.ls[i] = -INFINITY; L1.ls[i] = -INFINITY; }
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+  // descriptors: A = this warpgroup's 64 rows of the query image, B = ring stage 0; one k-step (two 8-column K-chunks)
+  // advances the start address by 2 * LBO bytes (the address field counts 16-byte units)
+  const uint64_t da0 = wgmma_desc(smem_u32(As) + (uint32_t)g * 8u * SBO, LBO, SBO);
+  const uint64_t db0 = wgmma_desc(smem_u32(Bs0), LBO, SBO);
+  constexpr uint32_t KSTEP16 = (2u * LBO) >> 4;
+  const uint32_t part16 = part_b >> 4;
+  const int n_visit = (int)(n_est + n_btiles), n_est_i = (int)n_est;
+  int32_t ctile = *start_tile;                 // candidate tile of the current sweep visit (cyclic walk)
+  int32_t cbase = ctile * CN + 2 * sl;
+  const int32_t n_bt = (int32_t)n_btiles;
+  int s = 0;
+  uint32_t ring_phase = 0;
+  mbar_wait(afull, 0);
+  for (int c = 0; c < n_visit; ++c) {
+    for (int p = 0; p < nsplit; ++p) {
+      mbar_wait(&full[s], ring_phase);
+      wgmma_fence();
+      const uint64_t da = da0 + (uint64_t)((uint32_t)(p * nks) * KSTEP16);
+      const uint64_t db = db0 + (uint64_t)((uint32_t)s * part16);
+      for (int j = 0; j < nks; ++j)
+        wgmma_m64n128k16_f16(acc, da + (uint64_t)((uint32_t)j * KSTEP16), db + (uint64_t)((uint32_t)j * KSTEP16), (p | j) != 0);
+      wgmma_commit();
+      wgmma_wait_all();
+      // this warp's reads of the stage are complete: the eighth arrival lets the producer refill it
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s]);
+      if (++s == nstage) { s = 0; ring_phase ^= 1u; }
     }
-#undef SB2_MPH
-    if (PHASES_M && blockIdx.x == gridDim.x / 2 && lane == 0) {
-      g_knn2_phase[0][6] = (unsigned long long)mph[0]; g_knn2_phase[0][7] = (unsigned long long)mph[1]; g_knn2_phase[1][6] = (unsigned long long)mph[2];
-    }
-    // teardown: every epilogue warp walks the visits in order, so the release of the last visit by all of them means
-    // every TMEM read of this CTA has completed
-    if (mma_visits > 0) {
-      const int bl = (mma_visits - 1) & 1;
-      mbar_wait(&tempty[bl], (uint32_t)(((mma_visits - 1) >> 1) & 1));
-    }
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(0u), "r"(512u) : "memory");
-  } else {
-    // ---------------- epilogue: thread <-> (query row, column quarter) ----------------
-    const int lgrp = warp & 3;              // TMEM lane quadrant this warp may access
-    const int cq = warp >> 2;               // column quarter 0..3 (the four warps of a quadrant: w, w+4, w+8, w+12)
-    const int row = lgrp * 32 + lane;
-    const int64_t ql = (int64_t)blockIdx.x * QM + row;  // local query index
-    const bool valid = ql < n_query;
-    constexpr int LS = 8 * NG, LM = NQUART * LS;
-    float* sc = cand_score + (valid ? ql : 0) * LM + cq * LS;
-    int32_t* id = cand_idx + (valid ? ql : 0) * LM + cq * LS;
-    SubList<NG> L;
-    L.tau = INFINITY;
-    if (valid) {
+    if (c == n_est_i) {
+      // start of the sweep proper: seed the sub-lists.  With an estimate phase the four sub-lists of a row (lanes
+      // lane ^ 1, ^ 2, ^ 3) are merged: the 6th largest of their 24 chunk maxima sits at about rank 6 * est_stride = 96
+      // of the row; without one the lists start cold (-inf).  Any value is safe: the certificate uses the final tau.
+      if (n_est_i > 0) {
+        float o0[EST_R], o1[EST_R];
 #pragma unroll
-      for (int i = 0; i < LS; ++i) id[i] = -1;
-    }
-    // During the estimate phase the EST_R running chunk maxima live in L.ls[0..EST_R) (the sub-list proper does not exist
-    // yet): one register array serves both phases.
-    static_assert(EST_R <= LS, "estimate aliases the list registers");
+        for (int i = 0; i < EST_R; ++i) { o0[i] = L0.ls[i]; o1[i] = L1.ls[i]; }
 #pragma unroll
-    for (int i = 0; i < LS; ++i) L.ls[i] = -INFINITY;
-    uint32_t v[32];
-    const uint32_t lane_base = tmem_base + ((uint32_t)(lgrp * 32) << 16) + (uint32_t)(cq * 64);
-    const int n_visit = mma_visits, n_est_i = (int)n_est;
-    int32_t ctile = *start_tile;                 // candidate tile of the current sweep visit (cyclic walk)
-    int32_t cbase = ctile * CN + cq * 64;
-    const int32_t n_bt = (int32_t)n_btiles;
-    const bool stamp = blockIdx.x == gridDim.x / 2 && warp == 2 && lane == 0;
-    unsigned long long st_c = 0, st_t = 0;
-    if (stamp) { st_c = clock64(); st_t = gtimer_ns(); }
-    constexpr bool NOSCAN = MODE == 1;
-    constexpr bool PHASES = MODE == 2;
-    long long ph[6] = {0, 0, 0, 0, 0, 0}, tp = 0;
-    const bool phw = PHASES && blockIdx.x == gridDim.x / 2 && (warp == 2 || warp == 5) && lane == 0  /* SMSP 2 (no service warp) and SMSP 1 (MMA issuer) */;
-    if (PHASES) tp = clock64();
-#define SB2_PH(i) if (PHASES) { const long long tn = clock64(); ph[i] += tn - tp; tp = tn; }
-    for (int c = 0; c < n_visit; ++c) {
-      const int b = c & 1;
-      mbar_wait(&tfull[b], (uint32_t)((c >> 1) & 1));
-      tc_fence_after();
-      SB2_PH(0)
-      const uint32_t taddr = lane_base + (uint32_t)(b * CN);
-      tmem_ld32_nowait(taddr, v);
-      tmem_wait_ld();
-      SB2_PH(1)
-      if (c == n_est_i) {
-        // start of the sweep proper: seed the sub-list.  With an estimate phase the four column quarters of a row are
-        // merged (the 6th largest of their 24 chunk maxima sits at about rank 6 * est_stride = 96 of the row);
-        // without one the lists start cold (-inf).  Any value is safe: the certificate uses the final tau.
-        if (n_est_i > 0) {
+        for (int o = 1; o < NSUB; ++o) {
 #pragma unroll
-          for (int i = 0; i < EST_R; ++i) est_x[(row * NQUART + cq) * EST_R + i] = L.ls[i];
-          named_bar_sync(1, NEPI * 32);
-#pragma unroll
-          for (int o = 1; o < NQUART; ++o) {
-            const int oq = (cq + o) & (NQUART - 1);
-#pragma unroll
-            for (int i = 0; i < EST_R; ++i) est_push(L.ls, est_x[(row * NQUART + oq) * EST_R + i]);
+          for (int i = 0; i < EST_R; ++i) {
+            est_push(L0.ls, __shfl_xor_sync(0xffffffffu, o0[i], o));
+            est_push(L1.ls, __shfl_xor_sync(0xffffffffu, o1[i], o));
           }
         }
-        const float t0 = valid ? L.ls[EST_R - 1] : INFINITY;  // rows past n_query never accept anything
-#pragma unroll
-        for (int i = 0; i < LS; ++i) L.ls[i] = t0;
-#pragma unroll
-        for (int g = 0; g < NG; ++g) L.gm[g] = t0;
-        L.tau = t0;
       }
-      const bool estimating = c < n_est_i;
-      if (!NOSCAN) { if (estimating) est_chunk(L.ls, v); else scan_chunk(L, id, v, cbase, n_points); }
-      SB2_PH(2)
-      tmem_ld32_nowait(taddr + 32u, v);
-      tmem_wait_ld();
-      SB2_PH(3)
-      // this warp's 64 columns have left TMEM: hand the buffer back (the 16th arrival lets the MMA warp refill it)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty[b]);
-      SB2_PH(4)
-      if (!NOSCAN) { if (estimating) est_chunk(L.ls, v); else scan_chunk(L, id, v, cbase + 32, n_points); }
-      SB2_PH(5)
-      if (!estimating) {
-        if ((c & 15) == 0 && warp == 0 && lane == 0) atomicAdd(&g_knn2_front, 1ull);   // 16 more visits of the pack
-        cbase += CN;
-        if (++ctile == n_bt) { ctile = 0; cbase = cq * 64; }
-      }
-    }
-#undef SB2_PH
-    if (phw) {
+      const float t0 = valid0 ? L0.ls[EST_R - 1] : INFINITY;  // rows past n_query never accept anything
+      const float t1 = valid1 ? L1.ls[EST_R - 1] : INFINITY;
 #pragma unroll
-      for (int i = 0; i < 6; ++i) g_knn2_phase[warp == 2 ? 0 : 1][i] = (unsigned long long)ph[i];
-    }
-    if (stamp) {
-      g_knn2_stamp[0] = clock64() - st_c;
-      g_knn2_stamp[1] = gtimer_ns() - st_t;
-      g_knn2_stamp[2] = (unsigned long long)n_visit;
-    }
-    if (valid) {
+      for (int i = 0; i < LS; ++i) { L0.ls[i] = t0; L1.ls[i] = t1; }
 #pragma unroll
-      for (int i = 0; i < LS; ++i) sc[i] = L.ls[i];
+      for (int gi = 0; gi < NG; ++gi) { L0.gm[gi] = t0; L1.gm[gi] = t1; }
+      L0.tau = t0;
+      L1.tau = t1;
+    }
+    uint32_t v0[32], v1[32];
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      v0[2 * i] = __float_as_uint(acc[4 * i]);
+      v0[2 * i + 1] = __float_as_uint(acc[4 * i + 1]);
+      v1[2 * i] = __float_as_uint(acc[4 * i + 2]);
+      v1[2 * i + 1] = __float_as_uint(acc[4 * i + 3]);
+    }
+    if (c < n_est_i) {
+      est_chunk(L0.ls, v0);
+      est_chunk(L1.ls, v1);
+    } else {
+      scan_chunk(L0, id0, v0, cbase, n_points);
+      scan_chunk(L1, id1, v1, cbase, n_points);
+      if ((c & 15) == 0 && warp == 0 && lane == 0) atomicAdd(&g_knn2_front, 1ull);   // 16 more visits of the pack
+      cbase += CN;
+      if (++ctile == n_bt) { ctile = 0; cbase = 2 * sl; }
     }
   }
-  // no CTA-wide barrier down here: code after the role branches would make ptxas treat the MMA warp's region as
-  // divergent (its operands then leave the uniform datapath).  The MMA warp tears TMEM down by itself.
+  if (valid0) {
+#pragma unroll
+    for (int i = 0; i < LS; ++i) sc0[i] = L0.ls[i];
+  }
+  if (valid1) {
+#pragma unroll
+    for (int i = 0; i < LS; ++i) sc1[i] = L1.ls[i];
+  }
 }
 
 }  // namespace
@@ -509,23 +410,21 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
 bool knn_tc2_supported(int d) { return 3 * d + 3 <= 512; }
 
 bool knn_tc2_shape(const sb2_ctx* ctx, int d, int terms, bool want_estimate, KnnTc2Shape* out) {
-  // one 128-row query image + a ring of candidate-image K-slices (256 rows each) in 227 KB; the K axis is staged in
-  // 1, 2, 4 or 8 slices, fewest first; at least 3 ring stages (2 when nothing else fits)
+  // one 128-row query image + a ring of candidate-image K-slices (128 rows each) in the opt-in shared memory of a
+  // block; the K axis is staged in 1, 2, 4 or 8 slices, fewest first; at least 3 ring stages (2 when nothing else fits)
   const size_t cap = ctx->prop.sharedMemPerBlockOptin;
   for (int min_st = 3; min_st >= 2; --min_st) {
     for (int ns = 1; ns <= 8; ns *= 2) {
       const int unit = 16 * ns;
       const int kp = ((terms * d + 3 + unit - 1) / unit) * unit;
       const size_t ta = (size_t)QM * kp * 2, part = (size_t)CN * kp * 2 / ns;
-      for (int est = want_estimate ? 1 : 0; est >= 0; --est) {
-        const size_t fixed = BAR_BYTES + ta + (est ? EST_BYTES : 0);
-        if (fixed + (size_t)min_st * part > cap) continue;
-        int nst = (int)((cap - fixed) / part);
-        if (nst > MAXST) nst = MAXST;
-        out->nsplit = ns; out->nstage = nst; out->kpad = kp; out->terms = terms; out->est = est;
-        out->smem = fixed + (size_t)nst * part;
-        return true;
-      }
+      const size_t fixed = BAR_BYTES + ta;
+      if (fixed + (size_t)min_st * part > cap) continue;
+      int nst = (int)((cap - fixed) / part);
+      if (nst > MAXST) nst = MAXST;
+      out->nsplit = ns; out->nstage = nst; out->kpad = kp; out->terms = terms; out->est = want_estimate ? 1 : 0;
+      out->smem = fixed + (size_t)nst * part;
+      return true;
     }
   }
   return false;
@@ -554,15 +453,14 @@ int32_t knn_tc2_build_images(sb2_ctx* ctx, const KnnTc2Shape& sh, const float* d
 }
 
 namespace {
-template <int NG, int MODE>
+template <int NG>
 cudaError_t launch2(unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B, int64_t n_tiles,
                     int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs, int32_t* ci) {
-  cudaError_t e = cudaFuncSetAttribute(knn_sweep2_kernel<NG, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
+  cudaError_t e = cudaFuncSetAttribute(knn_sweep2_kernel<NG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
   if (e != cudaSuccess) return e;
   const int nks = sh.kpad / 16 / sh.nsplit;
-  knn_sweep2_kernel<NG, MODE><<<grid, THREADS, sh.smem, st>>>(A, B, nks, sh.nsplit, sh.nstage, (uint32_t)(CN * sh.kpad * 2 / sh.nsplit) >> 4,
-                                                                (uint32_t)(QM * sh.kpad * 2) >> 4, (int)(n_tiles + n_est), n_tiles, n_est,
-                                                                est_stride, qtile0, n_query, n_points, cs, ci);
+  knn_sweep2_kernel<NG><<<grid, THREADS, sh.smem, st>>>(A, B, nks, sh.nsplit, sh.nstage, n_tiles, n_est, est_stride, qtile0, n_query,
+                                                        n_points, cs, ci);
   return cudaSuccess;
 }
 }  // namespace
@@ -583,42 +481,16 @@ int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnTc2Shape& sh, const __half* Aimg, i
   if (issued_flops) *issued_flops += 2.0 * (double)(q_ctas * QM) * (double)((n_tiles + n_est) * CN) * (double)sh.kpad;
   const unsigned grid = (unsigned)q_ctas;
   const int32_t np = (int32_t)n_points;
-  const char* ns_env = getenv("SB2_KNN2_NOSCAN");   // timing experiments: 1 = epilogue loads but does not examine, 2 = per-phase cycle stamps
-  const int mode = ns_env ? atoi(ns_env) : 0;
   {
     void* fp = nullptr;
     SB2_CUDA(cudaGetSymbolAddress(&fp, g_knn2_front));
     SB2_CUDA(cudaMemsetAsync(fp, 0, sizeof(unsigned long long), st));
   }
   cudaError_t le;
-#define SB2_L2(NGV, MODEV) launch2<NGV, MODEV>(grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, a_tile0, n_query, np, cand_score, cand_idx)
-  if (list_m == 64) le = mode == 1 ? SB2_L2(2, 1) : (mode == 2 ? SB2_L2(2, 2) : SB2_L2(2, 0));
-  else le = SB2_L2(4, 0);
-#undef SB2_L2
+  if (list_m == 64) le = launch2<2>(grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, a_tile0, n_query, np, cand_score, cand_idx);
+  else le = launch2<4>(grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, a_tile0, n_query, np, cand_score, cand_idx);
   SB2_CUDA(le);
   SB2_LAUNCH_CHECK(ctx);
-  if (getenv("SB2_KNN2_STAMP")) {
-    unsigned long long h[4] = {0, 0, 0, 0};
-    SB2_CUDA(cudaStreamSynchronize(st));
-    SB2_CUDA(cudaMemcpyFromSymbol(h, g_knn2_stamp, sizeof(h)));
-    if (h[2] > 0)
-      fprintf(stderr, "[knn2 stamp] grid %u, CTA %u: %llu visits, %.1f cycles/visit (tensor floor %d), SM clock under load %.0f MHz\n", grid,
-              grid / 2, h[2], (double)h[0] / (double)h[2], 4 * (sh.kpad / 16) * (CN / 2) / 4, 1e3 * (double)h[0] / (double)h[1]);
-    if (mode == 2 && h[2] > 0) {
-      unsigned long long p[2][8];
-      SB2_CUDA(cudaMemcpyFromSymbol(p, g_knn2_phase, sizeof(p)));
-      for (int w = 0; w < 2; ++w)
-        fprintf(stderr, "[knn2 phases] warp %d cycles/visit: wait tfull %.0f | ld0 %.0f | scan0 %.0f | ld1 %.0f | release %.0f | scan1 %.0f\n", w ? 5 : 2,
-                (double)p[w][0] / h[2], (double)p[w][1] / h[2], (double)p[w][2] / h[2], (double)p[w][3] / h[2], (double)p[w][4] / h[2], (double)p[w][5] / h[2]);
-      ;
-    }
-    if (mode == 2 && h[2] > 0) {
-      unsigned long long p[2][8];
-      SB2_CUDA(cudaMemcpyFromSymbol(p, g_knn2_phase, sizeof(p)));
-      fprintf(stderr, "[knn2 phases] MMA issuer cycles/visit: wait full (ring) %.0f | wait tempty (epilogue) %.0f | issue + commits %.0f\n",
-              (double)p[0][6] / h[2], (double)p[0][7] / h[2], (double)p[1][6] / h[2]);
-    }
-  }
   return SB2_OK;
 }
 

@@ -1,4 +1,4 @@
-// leiden.cu — Leiden community detection on a symmetric weighted CSR graph (sm_100a).
+// leiden.cu — Leiden community detection on a symmetric weighted CSR graph (sm_90a).
 //
 // Replaces leidenalg.find_partition(RBConfigurationVertexPartition) / igraph community_leiden as
 // called by the reference at src/scanpy/tools/_leiden.py:184-187,195-196 (and eliminates the Python

@@ -1,5 +1,5 @@
-// tc_ptx.cuh — thin inline-PTX wrappers (sm_100a): mbarriers, 1-D bulk (TMA) copies, tcgen05 fences / MMA / commit /
-// TMEM loads.  Shared by the tensor-core kNN sweep (knn_tc2.cu).
+// tc_ptx.cuh — thin inline-PTX wrappers (sm_90a): mbarriers, 1-D bulk (TMA) copies, warpgroup MMA (wgmma) on
+// shared-memory operands.  Shared by the tensor-core kNN sweep (knn_tc2.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -29,71 +29,52 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "r"(parity)
       : "memory");
 }
-// 1-D bulk async copy global -> shared (TMA engine, SASS UBLKCP), completion counted on an mbarrier
+// 1-D bulk async copy global -> shared (TMA engine), completion counted on an mbarrier
 __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                    smem_u32(dst)),
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// UMMA shared-memory descriptor, no swizzle, K-major (cute::UMMA::SmemDescriptor bit layout).
-// lbo = bytes between 8-column K-chunks, sbo = bytes between 8-row groups.
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+// wgmma shared-memory matrix descriptor, no swizzle ("interleave"), K-major operand made of 8x8 fp16 core matrices.
+// lbo = bytes between core matrices adjacent along K, sbo = bytes between 8-row groups (M / N direction).
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);            // start address   [0,14)
   d |= (uint64_t)((lbo >> 4) & 0x3FFFu) << 16;         // leading byte offset (K direction) [16,30)
   d |= (uint64_t)((sbo >> 4) & 0x3FFFu) << 32;         // stride byte offset (M/N direction) [32,46)
-  d |= (uint64_t)1 << 46;                              // descriptor version (Blackwell) [46,48)
-  return d;                                            // base_offset 0, lbo_mode 0, layout_type 0 = SWIZZLE_NONE
+  return d;                                            // base_offset 0, layout_type 0 = no swizzle
 }
-// instruction descriptor: D = F32, A = B = F16, both K-major, M = 128 (cute::UMMA::InstrDescriptor bit layout)
-__host__ __device__ constexpr uint32_t umma_idesc_f16_m128(uint32_t n) {
-  return (1u << 4) | ((n >> 3) << 17) | ((128u >> 4) << 24);
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// MMA issue.  The whole warp runs the (warp-uniform) issue loop and the single issuing thread is chosen INSIDE the asm
-// block (elect.sync): ptxas then keeps descriptors, TMEM addresses and loop counters on the uniform datapath and emits
-// back-to-back UTCHMMA.  Descriptors are (lo, hi) halves: only lo moves along K.
-template <bool ACC>
-__device__ __forceinline__ void umma_f16_elect(uint32_t tmem_d, uint32_t da_lo, uint32_t db_lo, uint32_t desc_hi, uint32_t idesc) {
+// D[64x128] (+)= A[64x16] B[128x16]^T, fp16 operands from shared memory (both K-major), fp32 accumulators in registers.
+// scale_d = 0 overwrites D.  Fragment of thread t of the warpgroup (warp w = t / 32, lane l): d[4i + 2h + e] is row
+// 16w + l/4 + 8h, column 8i + 2(l%4) + e.
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t da, uint64_t db, int scale_d) {
   asm volatile(
       "{\n"
-      ".reg .pred p, pe;\n"
-      ".reg .b64 da, db;\n"
-      "setp.ne.b32 p, %5, 0;\n"
-      "mov.b64 da, {%1, %3};\n"
-      "mov.b64 db, {%2, %3};\n"
-      "elect.sync _|pe, 0xffffffff;\n"
-      "@pe tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "r"(da_lo), "r"(db_lo), "r"(desc_hi), "r"(idesc), "n"(ACC ? 1 : 0)
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d)
       : "memory");
-}
-__device__ __forceinline__ void tc_commit_elect(uint64_t* bar) {
-  asm volatile(
-      "{\n"
-      ".reg .pred pe;\n"
-      "elect.sync _|pe, 0xffffffff;\n"
-      "@pe tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n"
-      "}\n" ::"r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n_threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n_threads) : "memory");
 }
 
 }  // namespace tcptx

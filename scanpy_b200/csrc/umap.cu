@@ -110,13 +110,11 @@ umap_epoch_kernel(int32_t n, const int64_t* __restrict__ indptr, const int32_t* 
 }
 
 
-// Measured and dropped (round 2, B200, 1.3M cells, 200 epochs; profiles/README.md): the kernel above runs at 4.6 active
-// threads per warp instruction (1.88 ms per epoch = 376 ms).  Two variants with EIGHT LANES per vertex - lane 0 the double
-// pull, lanes 1..7 the negative samples of a sampled edge, displacements summed by a shuffle tree - were built and passed
-// the quality gates, but were not faster: with every lane repeating the per-edge sampling test 681 ms, with the 8 lanes
-// testing 8 edges in parallel and serving the sampled ones together 391 ms.  The four groups of a warp still sit in
-// different edges, so the divergence only moves from lanes to groups; removing it needs forces that are simultaneous
-// across a vertex's edges (a different optimiser), not a different thread mapping.
+// The kernel above is divergence-bound (one vertex per lane, each lane in its own edge).  Giving a vertex EIGHT LANES -
+// lane 0 the double pull, lanes 1..7 the negative samples of a sampled edge, displacements summed by a shuffle tree - does
+// not remove that: the four groups of a warp still sit in different edges, so the divergence only moves from lanes to
+// groups; removing it needs forces that are simultaneous across a vertex's edges (a different optimiser), not a different
+// thread mapping.
 
 // per-dimension min / max (float atomics through the ordered-int trick)
 __device__ __forceinline__ int f2ord(float f) { const int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }

@@ -1,4 +1,4 @@
-"""`sc.pp.pca` and `sc.pp.neighbors` with scanpy's signatures, running on libscanpy_b200 (B200, sm_100a).
+"""`sc.pp.pca` and `sc.pp.neighbors` with scanpy's signatures, running on libscanpy_b200 (H100, sm_90a).
 
 Drop-in scope (SURVEY.md 8b): same argument names, same `.obsm/.varm/.obsp/.uns` write-backs, same
 exception types/messages where the reference's tests pin them.  Options whose arithmetic is not

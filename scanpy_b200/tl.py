@@ -1,4 +1,4 @@
-"""`sc.tl.leiden` with scanpy's signature, running on libscanpy_b200 (B200, sm_100a).
+"""`sc.tl.leiden` with scanpy's signature, running on libscanpy_b200 (H100, sm_90a).
 
 Reference: src/scanpy/tools/_leiden.py:55-268, src/scanpy/tools/_utils_clustering.py:16-50,
 src/scanpy/_utils/__init__.py:969-986.  The CUDA implementation (csrc/leiden.cu) optimises the same

@@ -18,7 +18,7 @@ from ._compat import as_csr_f32
 
 
 class B200KNNTransformer:
-    """Exact euclidean kNN on one B200 (hand-written sm_100a kernels, see csrc/knn.cu)."""
+    """Exact euclidean kNN on one H100 (hand-written sm_90a kernels, see csrc/knn.cu)."""
 
     def __init__(self, n_neighbors: int = 15, *, metric: str = "euclidean", **_ignored):
         if metric not in ("euclidean", "l2"):

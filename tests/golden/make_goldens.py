@@ -1,4 +1,4 @@
-"""Regenerate tests/golden/*.npz from the read-only reference checkout (run in the build container only).
+"""Regenerate tests/golden/* from a checkout of the reference (scverse/scanpy).
 
 Two sources, both owned by the reference (scverse/scanpy @ fabadb94):
 
@@ -9,7 +9,7 @@ Two sources, both owned by the reference (scverse/scanpy @ fabadb94):
    zstd): obsm/X_pca, obsp/distances, obsp/connectivities, obs/louvain, uns/neighbors params.
    Decoded with zipfile + libzstd via ctypes (zarr/anndata are not installed here).
 
-Usage:  python tests/golden/make_goldens.py   (writes next to this file)
+Usage:  python tests/golden/make_goldens.py <scanpy checkout>   (writes next to this file)
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ from pathlib import Path
 
 import numpy as np
 
-REF = Path("/root/reference")
+REF = Path(".")  # set from the command line by main()
 OUT = Path(__file__).resolve().parent
 
 
@@ -94,6 +94,10 @@ def read_zarr_array(z: zipfile.ZipFile, path: str) -> np.ndarray:
 
 
 def main() -> None:
+    import sys
+
+    global REF
+    REF = Path(sys.argv[1])
     pca_l = literals_from(REF / "tests/test_pca.py", {"A_list", "A_pca", "A_svd"})
     nb_l = literals_from(
         REF / "tests/test_neighbors.py",
@@ -158,6 +162,18 @@ def main() -> None:
         dispersions_norm=np.array([float(r["dispersions_norm"]) for r in rows]),
         highly_variable=np.array([r["highly_variable"] == "TRUE" for r in rows]))
     print("raw X", log_counts.shape, log_counts.nnz, "seurat rows", len(rows))
+
+    # --- the fixture's own zarr bytes, cut down to what the on-disk CSR reader test needs (the whole zip is 1.7 MB): the
+    # root and group metadata and every entry of layers/counts, last copy of each name (the zip holds appended rewrites)
+    keep = {}
+    for info in z.infolist():
+        name = info.filename
+        if name in ("zarr.json", "obsm/zarr.json", "layers/zarr.json") or name.startswith("layers/counts/"):
+            keep[name] = z.read(info)
+    with zipfile.ZipFile(OUT / "pbmc68k_counts.zarr.zip", "w", zipfile.ZIP_STORED) as zo:
+        for name, raw in keep.items():
+            zo.writestr(name, raw)
+    print("counts store", sorted(keep))
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""Parity ON the BASELINE.json configurations (run on the B200 box: `pytest -m gpu`).
+"""Parity ON the BASELINE.json configurations (need an H100: `pytest -m gpu`).
 
 configs[0]  pbmc3k-shaped 2700 x 1838 CSR (pbmc3k itself needs a download; SURVEY.md 8d prescribes the generator at
             that shape, K = 8, plus the in-tree pbmc68k fixture for real data - see test_gpu_parity.py)

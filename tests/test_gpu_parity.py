@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box: `pytest -m gpu`).  Every product call goes through the C ABI
+"""GPU parity tests (need an H100: `pytest -m gpu`).  Every product call goes through the C ABI
 (ctypes -> libscanpy_b200.so); the oracle (tests-only) is the checker.
 
 Bars (BASELINE.json north_star): X_pca within 1e-4 relative up to sign, identical kNN index sets,
@@ -144,8 +144,8 @@ def test_knn_golden_pbmc68k(pbmc68k_graph):
 
 @pytest.mark.parametrize("n,d,k", [(1, 3, 1), (5, 2, 5), (127, 7, 15), (129, 50, 15), (1000, 50, 30), (4097, 33, 10),
                                    (12345, 50, 15), (3000, 100, 30), (2000, 150, 8), (6000, 50, 30), (5000, 40, 45), (100, 8, 56),
-                                   # tile-shape boundaries of the tensor-core pass (knn_tc.cu: 256-query CTAs up to d = 57,
-                                   # then 128-query CTAs with the K axis staged in 1 / 2 / 4 slices)
+                                   # tile-shape boundaries of the tensor-core pass (knn_tc2.cu: the split-precision K axis is
+                                   # staged in 1 / 2 / 4 slices, switching at d = 74 and d = 117 with 227 KB of shared memory)
                                    (3000, 57, 15), (3000, 58, 15), (2500, 73, 40), (2500, 74, 15), (2500, 116, 15),
                                    (2500, 117, 30), (3000, 150, 56)])
 def test_knn_identical_index_sets(n, d, k):
@@ -172,14 +172,14 @@ def test_knn_threshold_estimate_and_tiers_agree_with_oracle(monkeypatch):
     c = rs.standard_normal((20, d)).astype(np.float32) * 4
     x = (c[rs.randint(0, 20, n)] + rs.standard_normal((n, d))).astype(np.float32)
     idx, dist, info = _ops.knn(x, k)
-    assert info["pass1_tensor"] == 2   # second-generation tensor sweep
+    assert info["pass1_tensor"] == 2   # tensor-core sweep
     rows = rs.choice(n, 1500, replace=False)
     oi, od2 = oknn.knn_exact_f64(x, rows, k)          # float64 brute force: "identical" means identical
     assert oknn.exact_set_mismatches(idx[rows], oi, od2, k).sum() == 0
     np.testing.assert_allclose(dist[rows][:, 1:], np.sqrt(od2[:, 1:k]), rtol=1e-6, atol=1e-7)
     for env in (dict(SB2_KNN_EST="0"), dict(SB2_KNN_TIERS="3"), dict(SB2_KNN_TIERS="3", SB2_KNN_EST="0"), dict(SB2_KNN_LIST="64"),
-                dict(SB2_KNN_SCAN_SLOTS="0"), dict(SB2_KNN_V="1"), dict(SB2_KNN_V="1", SB2_KNN_EST="0"), dict(SB2_KNN_PASS1="ffma")):
-        for key in ("SB2_KNN_EST", "SB2_KNN_TIERS", "SB2_KNN_LIST", "SB2_KNN_SCAN_SLOTS", "SB2_KNN_V", "SB2_KNN_PASS1"):
+                dict(SB2_KNN_SCAN_SLOTS="0"), dict(SB2_KNN_PASS1="ffma")):
+        for key in ("SB2_KNN_EST", "SB2_KNN_TIERS", "SB2_KNN_LIST", "SB2_KNN_SCAN_SLOTS", "SB2_KNN_PASS1"):
             monkeypatch.delenv(key, raising=False)
         for key, val in env.items():
             monkeypatch.setenv(key, val)
@@ -254,7 +254,7 @@ def test_knn_transformer_in_reference_pipeline_shape():
 def test_knn_tensor_score_error_within_bound():
     """MEASURES the tensor-core scores against float64 on the hardware and checks the rounding-error bound the exactness
     certificate rests on (knn_tc2_error_coefs + the measured fp16 residual norms): for every proposal (q, c) of a
-    cold-start sweep  |s_tcgen05 / s^2 - (q.c - |c|^2/2)| <= eps(q).  Adversarial magnitudes: data far from the origin
+    cold-start sweep  |s_tensor / s^2 - (q.c - |c|^2/2)| <= eps(q).  Adversarial magnitudes: data far from the origin
     (huge common offset), wide dynamic range across coordinates, every K-slice count (d 20 -> K 32, d 50 -> 64, d 100 ->
     terms 3: K 320 in two slices), both operand formats."""
     import torch

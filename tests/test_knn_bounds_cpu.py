@@ -1,5 +1,5 @@
-"""The exact-kNN certificate rests on rounding bounds for the tensor-core scores (scanpy_b200/csrc/knn_tc.cu:
-`knn_tc_error_coefs`, `knn_tc_prep_kernel`; scanpy_b200/csrc/knn.cu: `knn_rescore_kernel`).  This CPU test restates
+"""The exact-kNN certificate rests on rounding bounds for the tensor-core scores (scanpy_b200/csrc/knn_tc2.cu:
+`knn_tc2_error_coefs`, `knn_tc2_prep_kernel`; scanpy_b200/csrc/knn.cu: `knn_rescore_kernel`).  This CPU test restates
 the operand formats in numpy, emulates a PESSIMISTIC tensor pipe (exact fp16 x fp16 products, every 16-product
 group and every accumulator update truncated towards zero to fp32) and checks that the bounds the kernels use hold
 for every (query, candidate) pair tried - including data far from the origin, tiny and huge scales, sub-normal
