@@ -112,21 +112,47 @@ def csr_to_device(x):
 
 
 # ------------------------------------------------------------------------------------------ PCA
+def _pca_call(entry, ctx, args, n_rows, g: int, n_comps: int, *, mean: bool = True, extra=()):
+    """`entry(ctx.handle, *args, [X_pca,] components, variance, variance_ratio, [mean,] *extra, &info)` on fresh outputs ->
+    the result dict: X_pca [n_rows x n_comps] (None when n_rows is None: the entry writes no projection) and components on
+    the device, the rest on the host, then the solver statistics."""
+    torch = _torch()
+    out = dict(X_pca=None if n_rows is None else torch.empty((n_rows, n_comps), dtype=torch.float32, device="cuda"),
+               components=torch.empty((n_comps, g), dtype=torch.float32, device="cuda"),
+               variance=np.empty(n_comps, np.float64), variance_ratio=np.empty(n_comps, np.float64))
+    if mean:
+        out["mean"] = np.empty(g, np.float64)
+    info = PcaInfo()
+    check(entry(ctx.handle, *args, *(ptr(a) for a in out.values() if a is not None), *extra, byref(info)))
+    return dict(out, iterations=info.iterations, converged=bool(info.converged), max_rel_residual=info.max_rel_residual,
+                total_var=info.total_var)
+
+
+def _download_pca(out):
+    """X_pca and components to host arrays; the device X_pca stays resident for the next stage."""
+    d_x_pca = out["X_pca"]
+    out["X_pca"], out["components"] = _to_host(d_x_pca, out["components"])
+    RESIDENT.put(out["X_pca"], d_x_pca)
+    return out
+
+
 def pca_csr_device(ctx, d_indptr, d_indices, d_data, n: int, g: int, n_comps: int, *, solver: int = 0,
                    max_iter: int = 0, tol: float = 0.0, seed: int = 0, n_total: int | None = None):
+    args = (n, n if n_total is None else n_total, g, ptr(d_indptr), ptr(d_indices), ptr(d_data), n_comps, solver, max_iter, tol,
+            seed)
+    return _pca_call(ctx.lib.sb2_pca_csr_f32, ctx, args, n, g, n_comps)
+
+
+def _pca_stream_solve(ctx, n: int, g: int, stats, gram, n_comps: int, seed: int):
+    """Gram-route solve on the column statistics and Gram matrix that sb2_pca_stream_accumulate_f32 summed over all n rows
+    -> (result dict with X_pca None, and the projection operator proj, shift, l for sb2_pca_stream_project_f32)."""
     torch = _torch()
-    x_pca = torch.empty((n, n_comps), dtype=torch.float32, device="cuda")
-    comps = torch.empty((n_comps, g), dtype=torch.float32, device="cuda")
-    var = np.empty(n_comps, np.float64)
-    ratio = np.empty(n_comps, np.float64)
-    mean = np.empty(g, np.float64)
-    info = PcaInfo()
-    check(ctx.lib.sb2_pca_csr_f32(ctx.handle, n, n if n_total is None else n_total, g, ptr(d_indptr), ptr(d_indices),
-                                  ptr(d_data), n_comps, solver, max_iter, tol, seed, ptr(x_pca), ptr(comps),
-                                  ptr(var), ptr(ratio), ptr(mean), byref(info)))
-    return dict(X_pca=x_pca, components=comps, variance=var, variance_ratio=ratio, mean=mean,
-                iterations=info.iterations, converged=bool(info.converged), max_rel_residual=info.max_rel_residual,
-                total_var=info.total_var)
+    proj = torch.empty(g * 128, dtype=torch.float32, device="cuda")
+    shift = torch.empty(128, dtype=torch.float32, device="cuda")
+    l = c_int32()
+    out = _pca_call(ctx.lib.sb2_pca_stream_solve_f32, ctx, (n, g, ptr(stats), ptr(gram), n_comps, 0, 0.0, seed), None, g,
+                    n_comps, extra=(ptr(proj), ptr(shift), byref(l)))
+    return out, proj, shift, l.value
 
 
 OVERLAP_MIN_NNZ = 1 << 24   # below ~16.7M stored entries the upload is too short to be worth pipelining
@@ -181,24 +207,14 @@ def _pca_csr_overlapped(ctx, x, n_comps: int, seed: int, n_chunks: int = 8):
         d_ip.record_stream(main)
         check(ctx.lib.sb2_pca_stream_accumulate_f32(ctx.handle, r1 - r0, g, ptr(d_ip), ptr(d_indices[lo:hi]) if hi > lo else ptr(d_indices),
                                                     ptr(d_data[lo:hi]) if hi > lo else ptr(d_data), ptr(stats), ptr(gram)))
-    comps = torch.empty((n_comps, g), dtype=torch.float32, device="cuda")
-    proj = torch.empty(g * 128, dtype=torch.float32, device="cuda")
-    shift = torch.empty(128, dtype=torch.float32, device="cuda")
-    var = np.empty(n_comps, np.float64)
-    ratio = np.empty(n_comps, np.float64)
-    mean = np.empty(g, np.float64)
-    l = c_int32()
-    info = PcaInfo()
-    check(ctx.lib.sb2_pca_stream_solve_f32(ctx.handle, n, g, ptr(stats), ptr(gram), n_comps, 0, 0.0, seed, ptr(comps), ptr(var),
-                                           ptr(ratio), ptr(mean), ptr(proj), ptr(shift), byref(l), byref(info)))
+    out, proj, shift, l = _pca_stream_solve(ctx, n, g, stats, gram, n_comps, seed)
     main.wait_event(ev_all)
-    x_pca = torch.empty((n, n_comps), dtype=torch.float32, device="cuda")
-    check(ctx.lib.sb2_pca_stream_project_f32(ctx.handle, n, g, ptr(d_indptr), ptr(d_indices), ptr(d_data), n_comps, l.value, ptr(proj),
-                                             ptr(shift), ptr(x_pca)))
+    out["X_pca"] = torch.empty((n, n_comps), dtype=torch.float32, device="cuda")
+    check(ctx.lib.sb2_pca_stream_project_f32(ctx.handle, n, g, ptr(d_indptr), ptr(d_indices), ptr(d_data), n_comps, l, ptr(proj),
+                                             ptr(shift), ptr(out["X_pca"])))
     for t in (d_indptr, d_indices, d_data):
         t.record_stream(side)
-    return dict(X_pca=x_pca, components=comps, variance=var, variance_ratio=ratio, mean=mean, iterations=info.iterations,
-                converged=bool(info.converged), max_rel_residual=info.max_rel_residual, total_var=info.total_var)
+    return out
 
 
 _SIDE = {}
@@ -221,37 +237,19 @@ def pca_csr(x, n_comps: int, *, solver: int = 0, max_iter: int = 0, tol: float =
     min_nnz = int(os.environ.get("SB2_PCA_OVERLAP_MIN_NNZ", OVERLAP_MIN_NNZ))
     if (solver == 1 and max_iter == 0 and tol == 0.0 and x.nnz >= min_nnz and getattr(ctx, "n_ranks", 1) == 1
             and g >= 64 and os.environ.get("SB2_PCA_OVERLAP", "0") == "1"):
-        out = _pca_csr_overlapped(ctx, x, n_comps, seed)
-        d_x_pca = out["X_pca"]
-        out["X_pca"], out["components"] = _to_host(out["X_pca"], out["components"])
-        RESIDENT.put(out["X_pca"], d_x_pca)
-        return out
+        return _download_pca(_pca_csr_overlapped(ctx, x, n_comps, seed))
     d_indptr, d_indices, d_data = csr_to_device(x)
-    out = pca_csr_device(ctx, d_indptr, d_indices, d_data, n, g, n_comps, solver=solver, max_iter=max_iter, tol=tol,
-                         seed=seed)
-    d_x_pca = out["X_pca"]
-    out["X_pca"], out["components"] = _to_host(out["X_pca"], out["components"])
-    RESIDENT.put(out["X_pca"], d_x_pca)
-    return out
+    return _download_pca(pca_csr_device(ctx, d_indptr, d_indices, d_data, n, g, n_comps, solver=solver, max_iter=max_iter,
+                                        tol=tol, seed=seed))
 
 
 def tsvd_csr(x, n_comps: int, *, solver: int = 1, seed: int = 0, ctx=None):
     """Truncated SVD of a scipy CSR (no centring; `sc.pp.pca(zero_center=False)`): host arrays out, keys as `pca_csr`."""
-    torch = _torch()
     ctx = ctx or _abi.default_context()
     n, g = x.shape
     d_indptr, d_indices, d_data = csr_to_device(x)
-    x_pca = torch.empty((n, n_comps), dtype=torch.float32, device="cuda")
-    comps = torch.empty((n_comps, g), dtype=torch.float32, device="cuda")
-    var = np.empty(n_comps, np.float64)
-    ratio = np.empty(n_comps, np.float64)
-    info = PcaInfo()
-    check(ctx.lib.sb2_tsvd_csr_f32(ctx.handle, n, g, ptr(d_indptr), ptr(d_indices), ptr(d_data), n_comps, solver, 0, 0.0, seed,
-                                   ptr(x_pca), ptr(comps), ptr(var), ptr(ratio), byref(info)))
-    h_x, h_c = _to_host(x_pca, comps)
-    RESIDENT.put(h_x, x_pca)
-    return dict(X_pca=h_x, components=h_c, variance=var, variance_ratio=ratio, iterations=info.iterations,
-                converged=bool(info.converged), max_rel_residual=info.max_rel_residual, total_var=info.total_var)
+    args = (n, g, ptr(d_indptr), ptr(d_indices), ptr(d_data), n_comps, solver, 0, 0.0, seed)
+    return _download_pca(_pca_call(ctx.lib.sb2_tsvd_csr_f32, ctx, args, n, g, n_comps, mean=False))
 
 
 def pca_csr_chunked(x, n_comps: int, *, chunk_size: int, seed: int = 0, ctx=None):
@@ -278,25 +276,15 @@ def pca_csr_chunked(x, n_comps: int, *, chunk_size: int, seed: int = 0, ctx=None
 
     for r0, r1, dp, di, dd in chunks():
         check(ctx.lib.sb2_pca_stream_accumulate_f32(ctx.handle, r1 - r0, g, ptr(dp), ptr(di), ptr(dd), ptr(stats), ptr(gram)))
-    comps = torch.empty((n_comps, g), dtype=torch.float32, device="cuda")
-    proj = torch.empty(g * 128, dtype=torch.float32, device="cuda")
-    shift = torch.empty(128, dtype=torch.float32, device="cuda")
-    var = np.empty(n_comps, np.float64)
-    ratio = np.empty(n_comps, np.float64)
-    mean = np.empty(g, np.float64)
-    l = c_int32()
-    info = PcaInfo()
-    check(ctx.lib.sb2_pca_stream_solve_f32(ctx.handle, n, g, ptr(stats), ptr(gram), n_comps, 0, 0.0, seed, ptr(comps), ptr(var),
-                                           ptr(ratio), ptr(mean), ptr(proj), ptr(shift), byref(l), byref(info)))
-    x_pca = np.empty((n, n_comps), np.float32)
+    out, proj, shift, l = _pca_stream_solve(ctx, n, g, stats, gram, n_comps, seed)
+    out["X_pca"] = np.empty((n, n_comps), np.float32)
     for r0, r1, dp, di, dd in chunks():
         part = torch.empty((r1 - r0, n_comps), dtype=torch.float32, device="cuda")
-        check(ctx.lib.sb2_pca_stream_project_f32(ctx.handle, r1 - r0, g, ptr(dp), ptr(di), ptr(dd), n_comps, l.value, ptr(proj),
+        check(ctx.lib.sb2_pca_stream_project_f32(ctx.handle, r1 - r0, g, ptr(dp), ptr(di), ptr(dd), n_comps, l, ptr(proj),
                                                  ptr(shift), ptr(part)))
-        x_pca[r0:r1] = _to_host(part)
-    return dict(X_pca=x_pca, components=_to_host(comps), variance=var, variance_ratio=ratio, mean=mean,
-                iterations=info.iterations, converged=bool(info.converged), max_rel_residual=info.max_rel_residual,
-                total_var=info.total_var)
+        out["X_pca"][r0:r1] = _to_host(part)
+    out["components"] = _to_host(out["components"])
+    return out
 
 
 # ------------------------------------------------------------------------------------------ kNN

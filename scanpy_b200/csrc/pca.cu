@@ -15,9 +15,10 @@
 //                          RED.ADD.F32x4 each into one of 8 replicated fp32 copies of Z (L2 resident)
 //   csr_gram_kernel        G += x_r x_r^T (upper triangle), warp per row, fp64 REDs into L2-resident G
 //   small dense fp64 helpers (g x l blocks, l <= 128): A^T B, A*M, C*V, residual norms.
+//   rr_jacobi_kernel       the l x l Rayleigh-Ritz eigenproblem for l <= 64, one CTA (fp64).
 // Host side (C++ in this file): the block subspace iteration, CholeskyQR2 with an eigen-based
-// fallback for rank-deficient blocks, and a cyclic-Jacobi eigensolver for the l x l Rayleigh-Ritz
-// problem (l <= 128; fp64).  Centering never densifies X:  X_c B = X B - 1 (mu^T B) and, because
+// fallback for rank-deficient blocks, and a cyclic-Jacobi eigensolver for the l = 128 Rayleigh-Ritz
+// problem (fp64).  Centering never densifies X:  X_c B = X B - 1 (mu^T B) and, because
 // the columns of that product sum to zero, X_c^T (X_c B) = X^T (X B - 1 mu^T B).
 #include <math.h>
 #include <string.h>
@@ -628,27 +629,35 @@ struct Rng {
   }
 };
 
+// Per-call state of the PCA stages
 struct PcaWork {
   sb2_ctx* ctx;
   cudaStream_t st;
-  int g, l;
-  // operator data
+  int64_t n_total;  // rows over all ranks
+  int g, l;         // feature count padded to at least the block width l
+  int g_real;       // un-padded feature count
+  // operator (solver 1: dense Gram; solver 0: CSR SpMM passes)
   int solver;
-  int64_t n;
+  double* d_mu;     // [g_real] operator mean, all zeros without centring (the Gram operator pads it to g)
+  double* d_C;      // [g x g] (solver 1)
+  int64_t n;        // (solver 0)
   const int64_t* indptr;
   const int32_t* indices;
   const float* data;
-  double* d_mu;     // [g]
-  double* d_C;      // [g x g] (solver 1)
-  float* d_Bf;      // [g x l] fp32 copy of V
-  float* d_shift;   // [l]
   float* d_Y;       // [n x l]
   float* d_Zc;      // [ZT_COPIES x g x l]
+  // scratch
+  float* d_Bf;      // [g x l] fp32 copy of a block V (the projection U at the end)
+  float* d_shift;   // [l] mu^T V of that block
   double* d_S;      // [l x l]
   double* d_M;      // [l x l]
-  double* d_tmp;    // [g x l]
-  int g_real;       // un-padded feature count
+  double *d_Z, *d_tmp, *d_theta, *d_res;  // [g x l], [g x l], [l], [l]
   Rng* rng;         // refills rank-deficient blocks
+  // results
+  double* d_V;                // [g x l] Ritz vectors, columns by descending Ritz value
+  std::vector<double> theta;  // [l] Ritz values
+  double total_var0;          // sum of per-gene variances, ddof 0 (TruncatedSVD's ratio denominator)
+  sb2_pca_info stats;         // loop statistics and the ddof-1 total variance
 };
 
 int32_t launch_spmm(sb2_ctx* ctx, int64_t n, int l, const int64_t* indptr, const int32_t* indices, const float* data,
@@ -681,28 +690,19 @@ int32_t launch_spmm_t(sb2_ctx* ctx, int64_t n, int g, int l, const int64_t* indp
   return SB2_OK;
 }
 
-// S = A^T B (device, l x l), copied to host
-int32_t tsmm_host(PcaWork& w, const double* A, const double* B, std::vector<double>& hS) {
+// S = A^T B (device, l x l) in w.d_S, and copied to hS unless it is null
+int32_t tsmm(PcaWork& w, const double* A, const double* B, std::vector<double>* hS) {
   const int l = w.l;
   SB2_CUDA(cudaMemsetAsync(w.d_S, 0, sizeof(double) * l * l, w.st));
   tsmm_tn_kernel<<<(unsigned)ceil_div64(w.g, 32), 256, sizeof(double) * 2 * 32 * l, w.st>>>(A, B, w.g, l, w.d_S);
   SB2_LAUNCH_CHECK(w.ctx);
-  hS.resize((size_t)l * l);
-  SB2_CUDA(cudaMemcpyAsync(hS.data(), w.d_S, sizeof(double) * l * l, cudaMemcpyDeviceToHost, w.st));
+  if (!hS) return SB2_OK;
+  hS->resize((size_t)l * l);
+  SB2_CUDA(cudaMemcpyAsync(hS->data(), w.d_S, sizeof(double) * l * l, cudaMemcpyDeviceToHost, w.st));
   SB2_CUDA(cudaStreamSynchronize(w.st));
   return SB2_OK;
 }
-// A <- A * M (M host l x l)
-int32_t right_mult_inplace(PcaWork& w, double* A, const std::vector<double>& hM) {
-  const int l = w.l;
-  SB2_CUDA(cudaMemcpyAsync(w.d_M, hM.data(), sizeof(double) * l * l, cudaMemcpyHostToDevice, w.st));
-  right_mult_kernel<<<(unsigned)ceil_div64((int64_t)w.g * l, 256), 256, sizeof(double) * l * l, w.st>>>(A, w.d_M, w.g, l, l,
-                                                                                                  w.d_tmp);
-  SB2_LAUNCH_CHECK(w.ctx);
-  SB2_CUDA(cudaMemcpyAsync(A, w.d_tmp, sizeof(double) * (size_t)w.g * l, cudaMemcpyDeviceToDevice, w.st));
-  return SB2_OK;
-}
-// A <- A * M with M already on the device (l x l)
+// A <- A * M with M on the device (l x l)
 int32_t right_mult_device(PcaWork& w, double* A, const double* dM) {
   const int l = w.l;
   right_mult_kernel<<<(unsigned)ceil_div64((int64_t)w.g * l, 256), 256, sizeof(double) * l * l, w.st>>>(A, dM, w.g, l, l, w.d_tmp);
@@ -710,18 +710,36 @@ int32_t right_mult_device(PcaWork& w, double* A, const double* dM) {
   SB2_CUDA(cudaMemcpyAsync(A, w.d_tmp, sizeof(double) * (size_t)w.g * l, cudaMemcpyDeviceToDevice, w.st));
   return SB2_OK;
 }
+// A <- A * M (M host l x l)
+int32_t right_mult_inplace(PcaWork& w, double* A, const std::vector<double>& hM) {
+  SB2_CUDA(cudaMemcpyAsync(w.d_M, hM.data(), sizeof(double) * w.l * w.l, cudaMemcpyHostToDevice, w.st));
+  return right_mult_device(w, A, w.d_M);
+}
 size_t rr_jacobi_smem(int l) { return sizeof(double) * (2 * (size_t)l * (l + 1) + l + RRJ_THREADS) + sizeof(int) * l; }
-// Rayleigh-Ritz on the device: S = V^T Z, eigen-decomposition (rr_jacobi_kernel), V <- V W, Z <- Z W; d_theta receives the
-// Ritz values (descending).  Nothing travels to the host.
-int32_t rayleigh_ritz_device(PcaWork& w, double* V, double* Z, double* d_theta) {
+// Rayleigh-Ritz step: S = V^T Z, its eigenvectors W, V <- V W (Ritz vectors), Z <- Z W (A * Ritz vectors), d_theta <- Ritz
+// values (descending).  Blocks up to 64 wide solve S on the device (rr_jacobi_kernel) and nothing travels to the host; the
+// 128-wide block's two l x l matrices do not fit one CTA's shared memory, so its S goes through the host Jacobi.
+int32_t rayleigh_ritz(PcaWork& w, double* V, double* Z, double* d_theta) {
   const int l = w.l;
-  SB2_CUDA(cudaMemsetAsync(w.d_S, 0, sizeof(double) * l * l, w.st));
-  tsmm_tn_kernel<<<(unsigned)ceil_div64(w.g, 32), 256, sizeof(double) * 2 * 32 * l, w.st>>>(V, Z, w.g, l, w.d_S);
-  SB2_LAUNCH_CHECK(w.ctx);
-  rr_jacobi_kernel<<<1, RRJ_THREADS, rr_jacobi_smem(l), w.st>>>(w.d_S, l, w.d_M, d_theta);
-  SB2_LAUNCH_CHECK(w.ctx);
-  SB2_TRY(right_mult_device(w, V, w.d_M));
-  SB2_TRY(right_mult_device(w, Z, w.d_M));
+  if (l <= 64) {
+    SB2_TRY(tsmm(w, V, Z, nullptr));
+    rr_jacobi_kernel<<<1, RRJ_THREADS, rr_jacobi_smem(l), w.st>>>(w.d_S, l, w.d_M, d_theta);
+    SB2_LAUNCH_CHECK(w.ctx);
+    SB2_TRY(right_mult_device(w, V, w.d_M));
+    return right_mult_device(w, Z, w.d_M);
+  }
+  std::vector<double> T, theta, W;
+  SB2_TRY(tsmm(w, V, Z, &T));
+  for (int i = 0; i < l; ++i)  // symmetrise
+    for (int j = i + 1; j < l; ++j) {
+      const double a = 0.5 * (T[(size_t)i * l + j] + T[(size_t)j * l + i]);
+      T[(size_t)i * l + j] = T[(size_t)j * l + i] = a;
+    }
+  jacobi_eigh(T, l, theta, W);
+  sort_desc(theta, W, l);
+  SB2_TRY(right_mult_inplace(w, V, W));
+  SB2_TRY(right_mult_inplace(w, Z, W));
+  SB2_CUDA(cudaMemcpyAsync(d_theta, theta.data(), sizeof(double) * l, cudaMemcpyHostToDevice, w.st));
   return SB2_OK;
 }
 // orthonormalise the columns of A (g x l): CholeskyQR, twice; eigen-based fallback if rank deficient
@@ -731,7 +749,7 @@ int32_t orthonormalize(PcaWork& w, double* A) {
   for (int attempt = 0; attempt < 3; ++attempt) {
     std::vector<int> dropped;
     for (int pass = 0; pass < 2; ++pass) {
-      SB2_TRY(tsmm_host(w, A, A, S));
+      SB2_TRY(tsmm(w, A, A, &S));
       // column scaling first: after a Chebyshev filter the columns differ by many orders of magnitude
       // (each is amplified by p(theta_j)), which would make the Gram matrix numerically singular although the
       // columns are nearly orthogonal.  S' = D^-1/2 S D^-1/2 has a unit diagonal.
@@ -791,8 +809,21 @@ __global__ void mu_dot_kernel(const double* __restrict__ mu, const double* __res
   if (threadIdx.x == 0) shift[j] = (float)red[0];
 }
 
-int32_t apply_operator_spmm(PcaWork& w, const double* V, double* Z) {
+// Z = A_op * V  (V, Z device g x l fp64); A_op = X_c^T X_c summed over all ranks
+int32_t apply_operator(PcaWork& w, const double* V, double* Z) {
   const int g = w.g, l = w.l;
+  if (w.solver == 1) {
+    // split K so that the grid covers the machine about twice over (fp64 REDs merge the partial tiles)
+    const int row_tiles = (int)ceil_div64(g, DSA_T), col_tiles = (int)ceil_div64(l, DSA_T);
+    int ksplit = std::max(1, (2 * w.ctx->prop.multiProcessorCount) / (row_tiles * col_tiles));
+    ksplit = std::min(ksplit, (int)ceil_div64(g, 4 * DSA_K));
+    const int k_per_split = (int)ceil_div64(ceil_div64(g, ksplit), DSA_K) * DSA_K;
+    SB2_CUDA(cudaMemsetAsync(Z, 0, sizeof(double) * (size_t)g * l, w.st));
+    dense_sym_apply_kernel<<<dim3((unsigned)row_tiles, (unsigned)ceil_div64(g, k_per_split), (unsigned)col_tiles), 256, 0, w.st>>>(
+        w.d_C, V, g, l, k_per_split, Z);
+    SB2_LAUNCH_CHECK(w.ctx);
+    return SB2_OK;
+  }
   const int64_t len = (int64_t)g * l;
   f64_to_f32_kernel<<<(unsigned)ceil_div64(len, 256), 256, 0, w.st>>>(V, w.d_Bf, len);
   SB2_LAUNCH_CHECK(w.ctx);
@@ -800,25 +831,282 @@ int32_t apply_operator_spmm(PcaWork& w, const double* V, double* Z) {
   SB2_LAUNCH_CHECK(w.ctx);
   SB2_TRY(launch_spmm(w.ctx, w.n, l, w.indptr, w.indices, w.data, w.d_Bf, w.d_shift, w.d_Y, l, l));
   SB2_TRY(launch_spmm_t(w.ctx, w.n, g, l, w.indptr, w.indices, w.data, w.d_Y, w.d_Zc, Z));
-  SB2_TRY(sb2_comm_allreduce_f64(w.ctx, Z, len));
+  return sb2_comm_allreduce_f64(w.ctx, Z, len);
+}
+
+// ---------------------------------------------------------------------------------------------
+// host stages of the PCA entries
+// Shape checks, block width l (k + oversampling, one of the kernel-supported widths) and route.  g < l genes are padded to
+// w.g = l (all-zero genes, eigenvalue 0) and take the dense Gram route.
+int32_t init_work(sb2_ctx* ctx, int64_t n, int64_t n_total, int g, int k, int solver, PcaWork& w) {
+  SB2_CHECK_ARG(n >= 0 && n_total >= n && n_total >= 2 && g >= 1, "shape");
+  SB2_CHECK_ARG(k >= 1 && k < std::min<int64_t>(n_total, g), "n_components must be between 1 and min(n_samples, n_features)-1");
+  SB2_CHECK_ARG(k <= 120, "n_components <= 120");
+  SB2_CHECK_ARG(solver == 0 || solver == 1, "solver");
+  SB2_CUDA(cudaSetDevice(ctx->device));
+  const int l = (k + 8 <= 32) ? 32 : (k + 8 <= 64 ? 64 : 128);
+  w.ctx = ctx; w.st = ctx->stream; w.n_total = n_total; w.l = l;
+  w.g_real = g; w.g = std::max(g, l);
+  w.solver = g < l ? 1 : solver;
+  return SB2_OK;
+}
+// The scratch of the iteration, and w.d_mu [g] for the caller to fill.  Allocated after the column statistics and before the
+// operator: the order decides where the g x g Gram matrix lands in the memory pool, and csr_gram_kernel's fp64 REDs took
+// 84.1 instead of 82.1 ms (1.3M x 2000, H100 80GB HBM3 at 700 W) with this scratch allocated ahead of the statistics.
+int32_t alloc_scratch(PcaWork& w, ScratchScope& scr) {
+  const size_t l = w.l, blk = (size_t)w.g * l;
+  SB2_TRY(scr.alloc(&w.d_mu, (size_t)w.g_real));
+  SB2_TRY(scr.alloc(&w.d_S, l * l));
+  SB2_TRY(scr.alloc(&w.d_M, l * l));
+  SB2_TRY(scr.alloc(&w.d_V, blk));
+  SB2_TRY(scr.alloc(&w.d_Z, blk));
+  SB2_TRY(scr.alloc(&w.d_tmp, blk));
+  SB2_TRY(scr.alloc(&w.d_theta, l));
+  SB2_TRY(scr.alloc(&w.d_res, l));
+  return scr.alloc(&w.d_Bf, blk);
+}
+
+// d_stats [2g]: column sums, then sums of squares, over all n_total rows -> h_mean [g] and the total variances
+int32_t gene_moments(PcaWork& w, const double* d_stats, double* h_mean) {
+  const int g = w.g_real;
+  std::vector<double> hs(2 * (size_t)g);
+  SB2_CUDA(cudaMemcpyAsync(hs.data(), d_stats, sizeof(double) * 2 * g, cudaMemcpyDeviceToHost, w.st));
+  SB2_CUDA(cudaStreamSynchronize(w.st));
+  const double nt = (double)w.n_total;
+  for (int j = 0; j < g; ++j) {
+    const double mu = hs[j] / nt;
+    h_mean[j] = mu;
+    w.stats.total_var += (hs[g + j] - nt * mu * mu) / (nt - 1.0);  // per-gene variance, ddof=1 (_pca.py:727-729)
+    w.total_var0 += hs[g + j] / nt - mu * mu;
+  }
+  return SB2_OK;
+}
+// In-core entries: the gene moments of the CSR rows, column statistics summed over the ranks
+int32_t incore_moments(PcaWork& w, ScratchScope& scr, int64_t n, const int64_t* indptr, const int32_t* indices,
+                       const float* data, double* h_mean) {
+  const int g = w.g_real;
+  double* d_stats;
+  SB2_TRY(scr.alloc(&d_stats, (size_t)2 * g));
+  SB2_TRY(sb2_csr_col_stats(w.ctx, n, g, indptr, indices, data, d_stats, d_stats + g));
+  SB2_TRY(sb2_comm_allreduce_f64(w.ctx, d_stats, 2 * (int64_t)g));
+  return gene_moments(w, d_stats, h_mean);
+}
+
+// Gram operator w.d_C = G - n_total mu mu^T [w.g x w.g], from G = X^T X [g x g] summed over all ranks, zero for padding genes.
+// G is centred in place when it needs no padding and the caller hands it over (G_is_scratch); otherwise it is copied.
+int32_t gram_operator(PcaWork& w, ScratchScope& scr, const double* G, bool G_is_scratch) {
+  const int g = w.g_real, gp = w.g;
+  if (gp == g && G_is_scratch) {
+    w.d_C = const_cast<double*>(G);
+  } else {
+    SB2_TRY(scr.alloc(&w.d_C, (size_t)gp * gp));
+    SB2_CUDA(cudaMemsetAsync(w.d_C, 0, sizeof(double) * (size_t)gp * gp, w.st));
+    SB2_CUDA(cudaMemcpy2DAsync(w.d_C, sizeof(double) * gp, G, sizeof(double) * g, sizeof(double) * g, g,
+                               cudaMemcpyDeviceToDevice, w.st));
+  }
+  if (gp != g) {
+    double* mup;
+    SB2_TRY(scr.alloc(&mup, (size_t)gp));
+    SB2_CUDA(cudaMemsetAsync(mup, 0, sizeof(double) * gp, w.st));
+    SB2_CUDA(cudaMemcpyAsync(mup, w.d_mu, sizeof(double) * g, cudaMemcpyDeviceToDevice, w.st));
+    w.d_mu = mup;
+  }
+  center_gram_kernel<<<(unsigned)ceil_div64((int64_t)gp * gp, 256), 256, 0, w.st>>>(w.d_C, w.d_mu, (double)w.n_total, gp);
+  SB2_LAUNCH_CHECK(w.ctx);
+  return SB2_OK;
+}
+// In-core entries: the operator of w.solver over the CSR rows, once w.d_mu holds the mean (SpMM: buffers for X_c V, X^T Y)
+int32_t incore_operator(PcaWork& w, ScratchScope& scr, int64_t n, const int64_t* indptr, const int32_t* indices,
+                        const float* data) {
+  const int g = w.g_real, l = w.l;
+  if (w.solver == 1) {
+    double* G;
+    SB2_TRY(scr.alloc(&G, (size_t)g * g));
+    SB2_TRY(sb2_csr_gram(w.ctx, n, g, indptr, indices, data, G));
+    SB2_TRY(sb2_comm_allreduce_f64(w.ctx, G, (int64_t)g * g));
+    return gram_operator(w, scr, G, true);
+  }
+  w.n = n; w.indptr = indptr; w.indices = indices; w.data = data;
+  SB2_TRY(scr.alloc(&w.d_shift, (size_t)l));
+  SB2_TRY(scr.alloc(&w.d_Y, (size_t)std::max<int64_t>(n, 1) * l));
+  SB2_TRY(scr.alloc(&w.d_Zc, (size_t)ZT_COPIES * g * l));
   return SB2_OK;
 }
 
-// Z = A_op * V  (V, Z device g x l fp64); A_op = X_c^T X_c summed over all ranks
-int32_t apply_operator(PcaWork& w, const double* V, double* Z) {
-  if (w.solver == 1) {
-    // split K so that the grid covers the machine about twice over (fp64 REDs merge the partial tiles)
-    const int row_tiles = (int)ceil_div64(w.g, DSA_T), col_tiles = (int)ceil_div64(w.l, DSA_T);
-    int ksplit = std::max(1, (2 * w.ctx->prop.multiProcessorCount) / (row_tiles * col_tiles));
-    ksplit = std::min(ksplit, (int)ceil_div64(w.g, 4 * DSA_K));
-    const int k_per_split = (int)ceil_div64(ceil_div64(w.g, ksplit), DSA_K) * DSA_K;
-    SB2_CUDA(cudaMemsetAsync(Z, 0, sizeof(double) * (size_t)w.g * w.l, w.st));
-    dense_sym_apply_kernel<<<dim3((unsigned)row_tiles, (unsigned)ceil_div64(w.g, k_per_split), (unsigned)col_tiles), 256, 0, w.st>>>(
-        w.d_C, V, w.g, w.l, k_per_split, Z);
-    SB2_LAUNCH_CHECK(w.ctx);
-    return SB2_OK;
+// Block subspace iteration with Rayleigh-Ritz on the operator w applies, from a start block drawn from `seed` (the same on
+// every rank).  Leaves the Ritz vectors in w.d_V (columns by descending Ritz value), the Ritz values in w.theta and the loop
+// statistics in w.stats.
+int32_t subspace_iteration(PcaWork& w, ScratchScope& scr, int k, int max_iter, double tol, uint64_t seed) {
+  sb2_ctx* ctx = w.ctx;
+  cudaStream_t st = w.st;
+  const int g = w.g_real, gp = w.g, l = w.l;
+  if (max_iter <= 0) max_iter = w.solver == 1 ? 4000 : 300;
+  // goal: the residual the iteration aims for; tol: the residual that counts as converged.  With the default tolerance the
+  // SpMM route (fp32 passes) aims 4x below it: an eigenvector's error is about its residual over its spectral gap, so
+  // stopping at the first iterate under 2e-6 leaves the smaller kept components (relative gaps ~1e-2) near 1e-4, while
+  // the fp32 rounding floor is lower still.  Iterates that stall at the floor above the goal count as converged once
+  // they are under tol.
+  double goal = tol;
+  if (!(tol > 0.0)) {
+    tol = w.solver == 1 ? 1e-10 : 2e-6;
+    goal = w.solver == 1 ? tol : tol / 4.0;
   }
-  return apply_operator_spmm(w, V, Z);
+  const int64_t blk = (int64_t)gp * l;
+  double *d_V = w.d_V, *d_Z = w.d_Z, *d_theta = w.d_theta, *d_res = w.d_res, *P[3];
+  SB2_CUDA(cudaFuncSetAttribute(tsmm_tn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * 2 * 32 * l)));
+  SB2_CUDA(cudaFuncSetAttribute(right_mult_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * l * l)));
+  if (l <= 64) SB2_CUDA(cudaFuncSetAttribute(rr_jacobi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rr_jacobi_smem(l)));
+
+  Rng rng(seed);
+  w.rng = &rng;
+  {
+    std::vector<double> hv((size_t)blk, 0.0);
+    for (int r = 0; r < g; ++r)
+      for (int j = 0; j < l; ++j) hv[(size_t)r * l + j] = rng.normal();
+    SB2_CUDA(cudaMemcpyAsync(d_V, hv.data(), sizeof(double) * (size_t)blk, cudaMemcpyHostToDevice, st));
+    SB2_CUDA(cudaStreamSynchronize(st));
+  }
+  SB2_TRY(orthonormalize(w, d_V));
+  for (double*& p : P) SB2_TRY(scr.alloc(&p, (size_t)blk));
+
+  std::vector<double> hres(l);
+  std::vector<double>& theta = w.theta;
+  theta.resize(l);
+  int32_t &it = w.stats.iterations, &converged = w.stats.converged;
+  double& max_rel = w.stats.max_rel_residual;
+  int stalled = 0;
+  double prev_rel = 1e300;
+  // Chebyshev-filtered subspace iteration (Zhou & Saad): between two Rayleigh-Ritz steps the block is
+  // multiplied by a degree-m Chebyshev polynomial of A that is bounded on the unwanted interval
+  // [0, theta_l] (A is PSD; theta_l = smallest Ritz value of the block) and grows fast above it.
+  const int cheb_m = 10;
+  const unsigned lgrid = (unsigned)ceil_div64(blk, 256);
+  for (;;) {
+    SB2_TRY(apply_operator(w, d_V, d_Z));
+    ++it;
+    SB2_TRY(rayleigh_ritz(w, d_V, d_Z, d_theta));
+    SB2_CUDA(cudaMemsetAsync(d_res, 0, sizeof(double) * l, st));
+    residual_kernel<<<32, (1024 / l) * l, 0, st>>>(d_Z, d_V, d_theta, gp, l, d_res);
+    SB2_LAUNCH_CHECK(ctx);
+    if (ctx->n_ranks > 1) {
+      // one process per GPU: the loop-control scalars must be THE SAME on every rank (the fp64 REDs behind them are
+      // order-dependent, and a rank that leaves the loop alone would strand the others in the next all-reduce):
+      // rank 0's Ritz values and residuals are broadcast (zero-fill elsewhere + sum all-reduce)
+      if (ctx->rank != 0) {
+        SB2_CUDA(cudaMemsetAsync(d_theta, 0, sizeof(double) * l, st));
+        SB2_CUDA(cudaMemsetAsync(d_res, 0, sizeof(double) * l, st));
+      }
+      SB2_TRY(sb2_comm_allreduce_f64(ctx, d_theta, l));
+      SB2_TRY(sb2_comm_allreduce_f64(ctx, d_res, l));
+    }
+    // the Ritz values come back together with the residual norms (one sync)
+    SB2_CUDA(cudaMemcpyAsync(hres.data(), d_res, sizeof(double) * l, cudaMemcpyDeviceToHost, st));
+    SB2_CUDA(cudaMemcpyAsync(theta.data(), d_theta, sizeof(double) * l, cudaMemcpyDeviceToHost, st));
+    SB2_CUDA(cudaStreamSynchronize(st));
+    max_rel = 0.0;
+    const double th1 = std::max(theta[0], 1e-300);
+    for (int j = 0; j < k; ++j) max_rel = std::max(max_rel, sqrt(std::max(hres[j], 0.0)) / th1);
+    converged = max_rel <= tol && theta[k - 1] > 0.0;
+    if (max_rel <= goal && converged) break;
+    if (it >= max_iter) break;
+    // stagnation at the operator's rounding floor (fp32 SpMM passes): stop; converged iff under tol
+    if (it > 3 && max_rel > 0.97 * prev_rel) { if (++stalled >= 3) break; } else stalled = 0;
+    prev_rel = max_rel;
+    const double cut = theta[l - 1], top = theta[0];
+    // degree: the filter amplifies the top of the wanted spectrum by T_m(x0), x0 = (top - c)/e, relative to the
+    // cut; beyond ~1e7 the columns next to the cut drown in rounding noise of the dominant directions, so m is
+    // capped by acosh(1e7)/acosh(x0) (a wide spectrum gets a low degree, a flat one the full cheb_m)
+    int m_use = 0;
+    if (it >= 3 && cut > 0.0 && top > 1.0001 * cut) {
+      const double x0 = 2.0 * top / cut - 1.0;
+      m_use = std::min(cheb_m, (int)floor(acosh(1e7) / acosh(x0)));
+    }
+    if (m_use >= 2) {
+      const double e = 0.5 * cut, c = 0.5 * cut;
+      double sigma = e / (top - c);
+      const double sigma1 = sigma;
+      // Y1 = (sigma1/e) (A V - c V), reusing Z = A V from the Rayleigh-Ritz step
+      double *prev = P[0], *cur = P[1], *nxt = P[2];
+      SB2_CUDA(cudaMemcpyAsync(prev, d_V, sizeof(double) * (size_t)blk, cudaMemcpyDeviceToDevice, st));
+      lincomb3_kernel<<<lgrid, 256, 0, st>>>(blk, sigma1 / e, d_Z, -(sigma1 / e) * c, d_V, 0.0, d_V, cur);
+      SB2_LAUNCH_CHECK(ctx);
+      for (int i = 2; i <= m_use && it < max_iter; ++i) {
+        const double sigma2 = 1.0 / (2.0 / sigma1 - sigma);
+        SB2_TRY(apply_operator(w, cur, d_Z));
+        ++it;
+        lincomb3_kernel<<<lgrid, 256, 0, st>>>(blk, 2.0 * sigma2 / e, d_Z, -(2.0 * sigma2 / e) * c, cur, -(sigma * sigma2), prev, nxt);
+        SB2_LAUNCH_CHECK(ctx);
+        double* t = prev; prev = cur; cur = nxt; nxt = t;
+        sigma = sigma2;
+      }
+      SB2_CUDA(cudaMemcpyAsync(d_V, cur, sizeof(double) * (size_t)blk, cudaMemcpyDeviceToDevice, st));
+    } else {
+      SB2_CUDA(cudaMemcpyAsync(d_V, d_Z, sizeof(double) * (size_t)blk, cudaMemcpyDeviceToDevice, st));
+    }
+    SB2_TRY(orthonormalize(w, d_V));
+  }
+  return SB2_OK;
+}
+
+// Signs of svd_flip(u_based_decision=False) (sklearn/utils/extmath.py:974-981) on the Ritz vectors w.d_V (in place), the
+// components d_components [k x g] (rows beyond g in the padded space are all-zero genes and are dropped), and the float32
+// projection operator of X_pca = X U - 1 (mu^T U): U [g x l] in w.d_Bf, mu^T U [l] in a fresh w.d_shift.
+int32_t projection_operator(PcaWork& w, ScratchScope& scr, int k, float* d_components) {
+  const int g = w.g_real, l = w.l;
+  double *d_V = w.d_V, *d_am;
+  SB2_TRY(scr.alloc(&d_am, (size_t)l));
+  col_absmax_kernel<<<l, 256, 0, w.st>>>(d_V, w.g, l, d_am);
+  SB2_LAUNCH_CHECK(w.ctx);
+  std::vector<double> am(l), hsign(l);
+  SB2_CUDA(cudaMemcpyAsync(am.data(), d_am, sizeof(double) * l, cudaMemcpyDeviceToHost, w.st));
+  SB2_CUDA(cudaStreamSynchronize(w.st));
+  for (int j = 0; j < l; ++j) hsign[j] = am[j] < 0.0 ? -1.0 : 1.0;
+  SB2_CUDA(cudaMemcpyAsync(d_am, hsign.data(), sizeof(double) * l, cudaMemcpyHostToDevice, w.st));
+  // the first g rows of V (row-major, ld = l) are contiguous already
+  components_out_kernel<<<(unsigned)ceil_div64((int64_t)k * g, 256), 256, 0, w.st>>>(d_V, d_am, g, l, k, d_components);
+  SB2_LAUNCH_CHECK(w.ctx);
+  std::vector<double> Dg((size_t)l * l, 0.0);
+  for (int j = 0; j < l; ++j) Dg[(size_t)j * l + j] = hsign[j];
+  SB2_TRY(right_mult_inplace(w, d_V, Dg));
+  const int64_t len = (int64_t)g * l;
+  f64_to_f32_kernel<<<(unsigned)ceil_div64(len, 256), 256, 0, w.st>>>(d_V, w.d_Bf, len);
+  SB2_LAUNCH_CHECK(w.ctx);
+  SB2_TRY(scr.alloc(&w.d_shift, (size_t)l));
+  mu_dot_kernel<<<l, 256, 0, w.st>>>(w.d_mu, d_V, g, l, w.d_shift);
+  SB2_LAUNCH_CHECK(w.ctx);
+  return SB2_OK;
+}
+
+// PCA: explained_variance_ = S^2/(n-1) (_pca.py:760-779), the ratio against the ddof-1 total
+void centred_variance(const PcaWork& w, int k, double* h_var, double* h_var_ratio) {
+  for (int j = 0; j < k; ++j) {
+    const double ev = std::max(w.theta[j], 0.0) / ((double)w.n_total - 1.0);
+    h_var[j] = ev;
+    h_var_ratio[j] = w.stats.total_var > 0.0 ? ev / w.stats.total_var : 0.0;
+  }
+}
+// TruncatedSVD (sklearn/decomposition/_truncated_svd.py): explained_variance_ = np.var(X_transformed, axis=0) (ddof 0)
+// = theta_j / n - (mean of column j)^2, the column mean of X V being mu . v_j; the ratio against sum_g var_g (ddof 0)
+int32_t tsvd_variance(const PcaWork& w, int k, const double* h_mean, double* h_var, double* h_var_ratio) {
+  const int g = w.g_real, l = w.l;
+  std::vector<double> hV((size_t)w.g * l);
+  SB2_CUDA(cudaMemcpyAsync(hV.data(), w.d_V, sizeof(double) * hV.size(), cudaMemcpyDeviceToHost, w.st));
+  SB2_CUDA(cudaStreamSynchronize(w.st));
+  for (int j = 0; j < k; ++j) {
+    double m = 0.0;
+    for (int r = 0; r < g; ++r) m += h_mean[r] * hV[(size_t)r * l + j];
+    const double ev = std::max(w.theta[j], 0.0) / (double)w.n_total - m * m;
+    h_var[j] = ev;
+    h_var_ratio[j] = w.total_var0 > 0.0 ? ev / w.total_var0 : 0.0;
+  }
+  return SB2_OK;
+}
+
+// waits for the last stage and reports the statistics
+int32_t report(const PcaWork& w, sb2_pca_info* info) {
+  SB2_CUDA(cudaStreamSynchronize(w.st));
+  if (info) *info = w.stats;
+  return SB2_OK;
 }
 
 }  // namespace
@@ -856,7 +1144,6 @@ int32_t sb2_csr_col_stats(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_i
 int32_t sb2_spmm_csr(sb2_ctx* ctx, int64_t n, int32_t g, int32_t l, const int64_t* d_indptr, const int32_t* d_indices,
                      const float* d_data, const float* d_b, const float* d_shift, float* d_y) {
   SB2_CHECK_ARG(ctx && d_indptr && d_b && d_y, "null pointer");
-  (void)g;
   SB2_CUDA(cudaSetDevice(ctx->device));
   return launch_spmm(ctx, n, l, d_indptr, d_indices, d_data, d_b, d_shift, d_y, l, l);
 }
@@ -934,315 +1221,23 @@ int32_t sb2_csr_gram(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_indptr
   return SB2_OK;
 }
 
-// pre_stats / pre_gram (both or neither): column sums [g] + sums of squares [g] and the Gram matrix X^T X [g x g] of ALL
-// rows, accumulated by the caller (sb2_pca_stream_accumulate_f32); the CSR arguments are then unused and nothing is
-// projected.  d_proj_out [g x l] / d_shift_out [l] / *l_out: the float32 projection operator (sign-fixed Ritz vectors and
-// mu^T U) for sb2_pca_stream_project_f32.
-static int32_t pca_core(sb2_ctx* ctx, int64_t n, int64_t n_total, int32_t g, const int64_t* d_indptr,
-                        const int32_t* d_indices, const float* d_data, int32_t k, int32_t solver, int32_t max_iter,
-                        double tol, uint64_t seed, float* d_x_pca, float* d_components, double* h_var,
-                        double* h_var_ratio, double* h_mean, sb2_pca_info* info, const double* pre_stats,
-                        const double* pre_gram, float* d_proj_out, float* d_shift_out, int32_t* l_out, bool center = true) {
-  const bool streamed = pre_stats != nullptr;
-  SB2_CHECK_ARG(ctx && (streamed || (d_indptr && d_x_pca)) && d_components && h_var && h_var_ratio && h_mean, "null pointer");
-  SB2_CHECK_ARG(!streamed || (pre_gram && d_proj_out && d_shift_out && l_out), "streamed PCA needs the Gram matrix and the projection outputs");
-  if (streamed) solver = 1;
-  SB2_CHECK_ARG(n >= 0 && n_total >= n && n_total >= 2 && g >= 1, "shape");
-  SB2_CHECK_ARG(k >= 1 && k < std::min<int64_t>(n_total, g), "n_components must be between 1 and min(n_samples, n_features)-1");
-  SB2_CHECK_ARG(k <= 120, "n_components <= 120");
-  SB2_CHECK_ARG(solver == 0 || solver == 1, "solver");
-  SB2_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = ctx->stream;
-  ScratchScope scr(ctx);
-  // block width: k + oversampling, one of the kernel-supported widths
-  const int l = (k + 8 <= 32) ? 32 : (k + 8 <= 64 ? 64 : 128);
-  // tiny feature spaces: the block cannot be wider than g; the dense Gram route handles them
-  if (g < l) solver = 1;
-  if (max_iter <= 0) max_iter = solver == 1 ? 4000 : 300;
-  // goal: the residual the iteration aims for; tol: the residual that counts as converged.  With the default tolerance the
-  // SpMM route (fp32 passes) aims 4x below it: an eigenvector's error is about its residual over its spectral gap, so
-  // stopping at the first iterate under 2e-6 leaves the smaller kept components (relative gaps ~1e-2) near 1e-4, while
-  // the fp32 rounding floor is lower still.  Iterates that stall at the floor above the goal count as converged once
-  // they are under tol.
-  double goal = tol;
-  if (!(tol > 0.0)) {
-    tol = solver == 1 ? 1e-10 : 2e-6;
-    goal = solver == 1 ? tol : tol / 4.0;
-  }
-
-  PcaWork w{};
-  w.ctx = ctx; w.st = st; w.g = g; w.l = l; w.solver = solver; w.n = n;
-  w.indptr = d_indptr; w.indices = d_indices; w.data = d_data;
-
-  // ---- column statistics -> mean, total variance ----
-  double *d_sum, *d_sumsq;
-  SB2_TRY(scr.alloc(&d_sum, (size_t)2 * g));
-  d_sumsq = d_sum + g;
-  if (streamed) {
-    SB2_CUDA(cudaMemcpyAsync(d_sum, pre_stats, sizeof(double) * 2 * g, cudaMemcpyDeviceToDevice, st));
-  } else {
-    SB2_TRY(sb2_csr_col_stats(ctx, n, g, d_indptr, d_indices, d_data, d_sum, d_sumsq));
-    SB2_TRY(sb2_comm_allreduce_f64(ctx, d_sum, 2 * (int64_t)g));
-  }
-  std::vector<double> hs(2 * (size_t)g);
-  SB2_CUDA(cudaMemcpyAsync(hs.data(), d_sum, sizeof(double) * 2 * g, cudaMemcpyDeviceToHost, st));
-  SB2_CUDA(cudaStreamSynchronize(st));
-  double total_var = 0.0;
-  const double nt = (double)n_total;
-  for (int j = 0; j < g; ++j) {
-    const double mu = hs[j] / nt;
-    h_mean[j] = mu;
-    total_var += (hs[g + j] - nt * mu * mu) / (nt - 1.0);  // per-gene variance, ddof=1 (_pca.py:727-729)
-  }
-  SB2_TRY(scr.alloc(&w.d_mu, (size_t)g));
-  // zero_center=False (TruncatedSVD semantics): the operator is X^T X itself - the device copy of mu is all zeros, so neither
-  // the Gram centring nor the SpMM shift does anything; the true column means stay in h_mean for the variance formulas
-  double full_var0 = 0.0;   // sum of per-gene variances with ddof = 0 (TruncatedSVD.explained_variance_ratio_'s denominator)
-  for (int j = 0; j < g; ++j) full_var0 += hs[g + j] / nt - h_mean[j] * h_mean[j];
-  if (center) SB2_CUDA(cudaMemcpyAsync(w.d_mu, h_mean, sizeof(double) * g, cudaMemcpyHostToDevice, st));
-  else SB2_CUDA(cudaMemsetAsync(w.d_mu, 0, sizeof(double) * g, st));
-
-  const int gl = (g < l) ? g : l;  // effective block width for tiny g handled below
-  (void)gl;
-
-  // ---- operator setup ----
-  SB2_TRY(scr.alloc(&w.d_S, (size_t)l * l));
-  SB2_TRY(scr.alloc(&w.d_M, (size_t)l * l));
-  double *d_V, *d_Z, *d_theta, *d_res;
-  const int gp = std::max(g, l);  // pad tiny feature spaces with all-zero genes (eigenvalue 0)
-  w.g = gp;
-  SB2_TRY(scr.alloc(&d_V, (size_t)gp * l));
-  SB2_TRY(scr.alloc(&d_Z, (size_t)gp * l));
-  SB2_TRY(scr.alloc(&w.d_tmp, (size_t)gp * l));
-  SB2_TRY(scr.alloc(&d_theta, (size_t)l));
-  SB2_TRY(scr.alloc(&d_res, (size_t)l));
-  SB2_TRY(scr.alloc(&w.d_Bf, (size_t)gp * l));
-  if (solver == 1) {
-    SB2_TRY(scr.alloc(&w.d_C, (size_t)gp * gp));
-    if (streamed) {
-      SB2_CUDA(cudaMemsetAsync(w.d_C, 0, sizeof(double) * (size_t)gp * gp, st));
-      SB2_CUDA(cudaMemcpy2DAsync(w.d_C, sizeof(double) * gp, pre_gram, sizeof(double) * g, sizeof(double) * g, g,
-                                 cudaMemcpyDeviceToDevice, st));
-    } else if (gp == g) {
-      SB2_TRY(sb2_csr_gram(ctx, n, g, d_indptr, d_indices, d_data, w.d_C));
-    } else {
-      double* Gs;
-      SB2_TRY(scr.alloc(&Gs, (size_t)g * g));
-      SB2_TRY(sb2_csr_gram(ctx, n, g, d_indptr, d_indices, d_data, Gs));
-      SB2_CUDA(cudaMemsetAsync(w.d_C, 0, sizeof(double) * (size_t)gp * gp, st));
-      SB2_CUDA(cudaMemcpy2DAsync(w.d_C, sizeof(double) * gp, Gs, sizeof(double) * g, sizeof(double) * g, g,
-                                 cudaMemcpyDeviceToDevice, st));
-    }
-    if (!streamed) SB2_TRY(sb2_comm_allreduce_f64(ctx, w.d_C, (int64_t)gp * gp));
-    if (gp != g) {  // mu padded with zeros
-      double* mup;
-      SB2_TRY(scr.alloc(&mup, (size_t)gp));
-      SB2_CUDA(cudaMemsetAsync(mup, 0, sizeof(double) * gp, st));
-      SB2_CUDA(cudaMemcpyAsync(mup, w.d_mu, sizeof(double) * g, cudaMemcpyDeviceToDevice, st));
-      w.d_mu = mup;
-    }
-    center_gram_kernel<<<(unsigned)ceil_div64((int64_t)gp * gp, 256), 256, 0, st>>>(w.d_C, w.d_mu, nt, gp);
-    SB2_LAUNCH_CHECK(ctx);
-  } else {
-    SB2_TRY(scr.alloc(&w.d_shift, (size_t)l));
-    SB2_TRY(scr.alloc(&w.d_Y, (size_t)std::max<int64_t>(n, 1) * l));
-    SB2_TRY(scr.alloc(&w.d_Zc, (size_t)ZT_COPIES * g * l));
-  }
-  SB2_CUDA(cudaFuncSetAttribute(tsmm_tn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * 2 * 32 * l)));
-  SB2_CUDA(cudaFuncSetAttribute(right_mult_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * l * l)));
-  if (l <= 64) SB2_CUDA(cudaFuncSetAttribute(rr_jacobi_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rr_jacobi_smem(l)));
-
-  // ---- start block (identical on every rank: same seed) ----
-  Rng rng(seed);
-  w.rng = &rng;
-  w.g_real = g;
-  {
-    std::vector<double> hv((size_t)gp * l, 0.0);
-    for (int r = 0; r < g; ++r)
-      for (int j = 0; j < l; ++j) hv[(size_t)r * l + j] = rng.normal();
-    SB2_CUDA(cudaMemcpyAsync(d_V, hv.data(), sizeof(double) * (size_t)gp * l, cudaMemcpyHostToDevice, st));
-    SB2_CUDA(cudaStreamSynchronize(st));
-  }
-  SB2_TRY(orthonormalize(w, d_V));
-
-  // ---- block subspace iteration with Rayleigh-Ritz ----
-  std::vector<double> T, theta, W, hres(l);
-  int it = 0, converged = 0;
-  double max_rel = 1e300, prev_rel = 1e300;
-  int stalled = 0;
-  // Chebyshev-filtered subspace iteration (Zhou & Saad): between two Rayleigh-Ritz steps the block is
-  // multiplied by a degree-m Chebyshev polynomial of A that is bounded on the unwanted interval
-  // [0, theta_l] (A is PSD; theta_l = smallest Ritz value of the block) and grows fast above it.
-  const int cheb_m = 10;
-  const int64_t blk = (int64_t)gp * l;
-  double *P0, *P1, *P2;
-  SB2_TRY(scr.alloc(&P0, (size_t)blk));
-  SB2_TRY(scr.alloc(&P1, (size_t)blk));
-  SB2_TRY(scr.alloc(&P2, (size_t)blk));
-  const unsigned lgrid = (unsigned)ceil_div64(blk, 256);
-  for (;;) {
-    SB2_TRY(apply_operator(w, d_V, d_Z));
-    ++it;
-    {
-      if (l <= 64) {
-        // Rayleigh-Ritz entirely on the device; the Ritz values come back together with the residual norms (one sync)
-        SB2_TRY(rayleigh_ritz_device(w, d_V, d_Z, d_theta));
-      } else {
-        SB2_TRY(tsmm_host(w, d_V, d_Z, T));
-        for (int i = 0; i < l; ++i)  // symmetrise
-          for (int j = i + 1; j < l; ++j) {
-            const double a = 0.5 * (T[(size_t)i * l + j] + T[(size_t)j * l + i]);
-            T[(size_t)i * l + j] = T[(size_t)j * l + i] = a;
-          }
-        jacobi_eigh(T, l, theta, W);
-        sort_desc(theta, W, l);
-        SB2_TRY(right_mult_inplace(w, d_V, W));  // V <- Ritz vectors
-        SB2_TRY(right_mult_inplace(w, d_Z, W));  // Z <- A * Ritz vectors
-        SB2_CUDA(cudaMemcpyAsync(d_theta, theta.data(), sizeof(double) * l, cudaMemcpyHostToDevice, st));
-      }
-      SB2_CUDA(cudaMemsetAsync(d_res, 0, sizeof(double) * l, st));
-      {
-        const int threads = (1024 / l) * l;
-        residual_kernel<<<32, threads, 0, st>>>(d_Z, d_V, d_theta, gp, l, d_res);
-        SB2_LAUNCH_CHECK(ctx);
-      }
-      if (ctx->n_ranks > 1) {
-        // one process per GPU: the loop-control scalars must be THE SAME on every rank (the fp64 REDs behind them are
-        // order-dependent, and a rank that leaves the loop alone would strand the others in the next all-reduce):
-        // rank 0's Ritz values and residuals are broadcast (zero-fill elsewhere + sum all-reduce)
-        if (ctx->rank != 0) {
-          SB2_CUDA(cudaMemsetAsync(d_theta, 0, sizeof(double) * l, st));
-          SB2_CUDA(cudaMemsetAsync(d_res, 0, sizeof(double) * l, st));
-        }
-        SB2_TRY(sb2_comm_allreduce_f64(ctx, d_theta, l));
-        SB2_TRY(sb2_comm_allreduce_f64(ctx, d_res, l));
-      }
-      SB2_CUDA(cudaMemcpyAsync(hres.data(), d_res, sizeof(double) * l, cudaMemcpyDeviceToHost, st));
-      if (l <= 64 || ctx->n_ranks > 1) {
-        theta.resize(l);
-        SB2_CUDA(cudaMemcpyAsync(theta.data(), d_theta, sizeof(double) * l, cudaMemcpyDeviceToHost, st));
-      }
-      SB2_CUDA(cudaStreamSynchronize(st));
-      max_rel = 0.0;
-      const double th1 = std::max(theta[0], 1e-300);
-      for (int j = 0; j < k; ++j) max_rel = std::max(max_rel, sqrt(std::max(hres[j], 0.0)) / th1);
-      converged = max_rel <= tol && theta[k - 1] > 0.0;
-      if (max_rel <= goal && converged) break;
-      if (it >= max_iter) break;
-      // stagnation at the operator's rounding floor (fp32 SpMM passes): stop; converged iff under tol
-      if (it > 3 && max_rel > 0.97 * prev_rel) { if (++stalled >= 3) break; } else stalled = 0;
-      prev_rel = max_rel;
-    }
-    const double cut = theta[l - 1], top = theta[0];
-    // degree: the filter amplifies the top of the wanted spectrum by T_m(x0), x0 = (top - c)/e, relative to the
-    // cut; beyond ~1e7 the columns next to the cut drown in rounding noise of the dominant directions, so m is
-    // capped by acosh(1e7)/acosh(x0) (a wide spectrum gets a low degree, a flat one the full cheb_m)
-    int m_use = 0;
-    if (it >= 3 && cut > 0.0 && top > 1.0001 * cut) {
-      const double x0 = 2.0 * top / cut - 1.0;
-      m_use = std::min(cheb_m, (int)floor(acosh(1e7) / acosh(x0)));
-    }
-    if (m_use >= 2) {
-      const double e = 0.5 * cut, c = 0.5 * cut;
-      double sigma = e / (top - c);
-      const double sigma1 = sigma;
-      // Y1 = (sigma1/e) (A V - c V), reusing Z = A V from the Rayleigh-Ritz step
-      double *prev = P0, *cur = P1, *nxt = P2;
-      SB2_CUDA(cudaMemcpyAsync(prev, d_V, sizeof(double) * (size_t)blk, cudaMemcpyDeviceToDevice, st));
-      lincomb3_kernel<<<lgrid, 256, 0, st>>>(blk, sigma1 / e, d_Z, -(sigma1 / e) * c, d_V, 0.0, d_V, cur);
-      SB2_LAUNCH_CHECK(ctx);
-      for (int i = 2; i <= m_use && it < max_iter; ++i) {
-        const double sigma2 = 1.0 / (2.0 / sigma1 - sigma);
-        SB2_TRY(apply_operator(w, cur, d_Z));
-        ++it;
-        lincomb3_kernel<<<lgrid, 256, 0, st>>>(blk, 2.0 * sigma2 / e, d_Z, -(2.0 * sigma2 / e) * c, cur, -(sigma * sigma2), prev, nxt);
-        SB2_LAUNCH_CHECK(ctx);
-        double* t = prev; prev = cur; cur = nxt; nxt = t;
-        sigma = sigma2;
-      }
-      SB2_CUDA(cudaMemcpyAsync(d_V, cur, sizeof(double) * (size_t)blk, cudaMemcpyDeviceToDevice, st));
-    } else {
-      SB2_CUDA(cudaMemcpyAsync(d_V, d_Z, sizeof(double) * (size_t)blk, cudaMemcpyDeviceToDevice, st));
-    }
-    SB2_TRY(orthonormalize(w, d_V));
-  }
-  // d_V now holds Ritz vectors (columns, descending theta)
-
-  // ---- sign convention: svd_flip(u_based_decision=False) (sklearn/utils/extmath.py:974-981) ----
-  std::vector<double> hsign(l, 1.0);
-  {
-    double* d_am;
-    SB2_TRY(scr.alloc(&d_am, (size_t)l));
-    col_absmax_kernel<<<l, 256, 0, st>>>(d_V, gp, l, d_am);
-    SB2_LAUNCH_CHECK(ctx);
-    std::vector<double> am(l);
-    SB2_CUDA(cudaMemcpyAsync(am.data(), d_am, sizeof(double) * l, cudaMemcpyDeviceToHost, st));
-    SB2_CUDA(cudaStreamSynchronize(st));
-    for (int j = 0; j < l; ++j) hsign[j] = am[j] < 0.0 ? -1.0 : 1.0;
-    SB2_CUDA(cudaMemcpyAsync(d_am, hsign.data(), sizeof(double) * l, cudaMemcpyHostToDevice, st));
-    // components_ = Vt (k x g)
-    // (rows beyond g in the padded space are all-zero genes and are dropped)
-    {
-      // compact U (gp x l) -> first g rows are contiguous already (row-major, ld = l)
-      components_out_kernel<<<(unsigned)ceil_div64((int64_t)k * g, 256), 256, 0, st>>>(d_V, d_am, g, l, k, d_components);
-      SB2_LAUNCH_CHECK(ctx);
-    }
-    // ---- X_pca = X * U - 1 * (mu^T U), U = sign-fixed Ritz vectors ----
-    // scale columns by sign, convert to fp32 (g x l), project with the SpMM kernel
-    std::vector<double> Dg((size_t)l * l, 0.0);
-    for (int j = 0; j < l; ++j) Dg[(size_t)j * l + j] = hsign[j];
-    SB2_TRY(right_mult_inplace(w, d_V, Dg));
-    const int64_t len = (int64_t)g * l;
-    f64_to_f32_kernel<<<(unsigned)ceil_div64(len, 256), 256, 0, st>>>(d_V, w.d_Bf, len);
-    SB2_LAUNCH_CHECK(ctx);
-    float* d_shift;
-    SB2_TRY(scr.alloc(&d_shift, (size_t)l));
-    mu_dot_kernel<<<l, 256, 0, st>>>(w.d_mu, d_V, g, l, d_shift);
-    SB2_LAUNCH_CHECK(ctx);
-    if (streamed) {
-      SB2_CUDA(cudaMemcpyAsync(d_proj_out, w.d_Bf, sizeof(float) * (size_t)g * l, cudaMemcpyDeviceToDevice, st));
-      SB2_CUDA(cudaMemcpyAsync(d_shift_out, d_shift, sizeof(float) * l, cudaMemcpyDeviceToDevice, st));
-      *l_out = l;
-    } else {
-      SB2_TRY(launch_spmm(ctx, n, l, d_indptr, d_indices, d_data, w.d_Bf, d_shift, d_x_pca, k, k));
-    }
-  }
-  if (center) {
-    for (int j = 0; j < k; ++j) {
-      const double ev = std::max(theta[j], 0.0) / (nt - 1.0);  // explained_variance_ = S^2/(n-1) (_pca.py:760-779)
-      h_var[j] = ev;
-      h_var_ratio[j] = total_var > 0.0 ? ev / total_var : 0.0;
-    }
-  } else {
-    // TruncatedSVD (sklearn/decomposition/_truncated_svd.py): explained_variance_ = np.var(X_transformed, axis=0) (ddof 0)
-    // = theta_j / n - (mean of column j)^2, the column mean of X V being mu . v_j; ratio against sum_g var_g (ddof 0)
-    std::vector<double> hV((size_t)gp * l);
-    SB2_CUDA(cudaMemcpyAsync(hV.data(), d_V, sizeof(double) * (size_t)gp * l, cudaMemcpyDeviceToHost, st));
-    SB2_CUDA(cudaStreamSynchronize(st));
-    for (int j = 0; j < k; ++j) {
-      double m = 0.0;
-      for (int r = 0; r < g; ++r) m += h_mean[r] * hV[(size_t)r * l + j];
-      const double ev = std::max(theta[j], 0.0) / nt - m * m;
-      h_var[j] = ev;
-      h_var_ratio[j] = full_var0 > 0.0 ? ev / full_var0 : 0.0;
-    }
-  }
-  SB2_CUDA(cudaStreamSynchronize(st));
-  if (info) {
-    info->iterations = it;
-    info->converged = converged;
-    info->max_rel_residual = max_rel;
-    info->total_var = total_var;
-  }
-  return SB2_OK;
-}
-
 int32_t sb2_pca_csr_f32(sb2_ctx* ctx, int64_t n, int64_t n_total, int32_t g, const int64_t* d_indptr,
                         const int32_t* d_indices, const float* d_data, int32_t k, int32_t solver, int32_t max_iter,
                         double tol, uint64_t seed, float* d_x_pca, float* d_components, double* h_var,
                         double* h_var_ratio, double* h_mean, sb2_pca_info* info) {
-  return pca_core(ctx, n, n_total, g, d_indptr, d_indices, d_data, k, solver, max_iter, tol, seed, d_x_pca, d_components, h_var,
-                  h_var_ratio, h_mean, info, nullptr, nullptr, nullptr, nullptr, nullptr);
+  SB2_CHECK_ARG(ctx && d_indptr && d_x_pca && d_components && h_var && h_var_ratio && h_mean, "null pointer");
+  PcaWork w{};
+  SB2_TRY(init_work(ctx, n, n_total, g, k, solver, w));
+  ScratchScope scr(ctx);
+  SB2_TRY(incore_moments(w, scr, n, d_indptr, d_indices, d_data, h_mean));
+  SB2_TRY(alloc_scratch(w, scr));
+  SB2_CUDA(cudaMemcpyAsync(w.d_mu, h_mean, sizeof(double) * g, cudaMemcpyHostToDevice, w.st));
+  SB2_TRY(incore_operator(w, scr, n, d_indptr, d_indices, d_data));
+  SB2_TRY(subspace_iteration(w, scr, k, max_iter, tol, seed));
+  SB2_TRY(projection_operator(w, scr, k, d_components));
+  SB2_TRY(launch_spmm(ctx, n, w.l, d_indptr, d_indices, d_data, w.d_Bf, w.d_shift, d_x_pca, k, k));
+  centred_variance(w, k, h_var, h_var_ratio);
+  return report(w, info);
 }
 
 // sc.pp.pca(zero_center=False): sklearn TruncatedSVD (src/scanpy/preprocessing/_pca/__init__.py:309-336) - top-k singular
@@ -1251,10 +1246,22 @@ int32_t sb2_tsvd_csr_f32(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_in
                          const float* d_data, int32_t k, int32_t solver, int32_t max_iter, double tol, uint64_t seed,
                          float* d_x_pca, float* d_components, double* h_var, double* h_var_ratio, sb2_pca_info* info) {
   SB2_CHECK_ARG(ctx && ctx->n_ranks == 1, "sb2_tsvd_csr_f32 is single-rank");
-  SB2_CHECK_ARG(g >= 1, "g");
-  std::vector<double> mean((size_t)g);
-  return pca_core(ctx, n, n, g, d_indptr, d_indices, d_data, k, solver, max_iter, tol, seed, d_x_pca, d_components, h_var,
-                  h_var_ratio, mean.data(), info, nullptr, nullptr, nullptr, nullptr, nullptr, false);
+  SB2_CHECK_ARG(d_indptr && d_x_pca && d_components && h_var && h_var_ratio, "null pointer");
+  PcaWork w{};
+  SB2_TRY(init_work(ctx, n, n, g, k, solver, w));
+  ScratchScope scr(ctx);
+  std::vector<double> h_mean((size_t)g);
+  SB2_TRY(incore_moments(w, scr, n, d_indptr, d_indices, d_data, h_mean.data()));
+  SB2_TRY(alloc_scratch(w, scr));
+  // the operator is X^T X itself: with an all-zero device mean neither the Gram centring nor the SpMM shift does anything;
+  // the true column means stay on the host for the variance formula
+  SB2_CUDA(cudaMemsetAsync(w.d_mu, 0, sizeof(double) * g, w.st));
+  SB2_TRY(incore_operator(w, scr, n, d_indptr, d_indices, d_data));
+  SB2_TRY(subspace_iteration(w, scr, k, max_iter, tol, seed));
+  SB2_TRY(projection_operator(w, scr, k, d_components));
+  SB2_TRY(launch_spmm(ctx, n, w.l, d_indptr, d_indices, d_data, w.d_Bf, w.d_shift, d_x_pca, k, k));
+  SB2_TRY(tsvd_variance(w, k, h_mean.data(), h_var, h_var_ratio));
+  return report(w, info);
 }
 
 // ---- out-of-core / chunked PCA (sc.pp.pca(chunked=True), src/scanpy/preprocessing/_pca/__init__.py:245-271) ----
@@ -1287,11 +1294,22 @@ int32_t sb2_pca_stream_solve_f32(sb2_ctx* ctx, int64_t n_total, int32_t g, const
                                  int32_t k, int32_t max_iter, double tol, uint64_t seed, float* d_components, double* h_var,
                                  double* h_var_ratio, double* h_mean, float* d_proj, float* d_shift, int32_t* h_l,
                                  sb2_pca_info* info) {
-  SB2_CHECK_ARG(d_stats && d_gram && d_proj && d_shift && h_l, "null pointer");
-  SB2_CHECK_ARG(n_total >= 2 && g >= 1, "shape");
-  SB2_CHECK_ARG(k >= 1 && k < std::min<int64_t>(n_total, g), "n_components must be between 1 and min(n_samples, n_features)-1");
-  return pca_core(ctx, 0, n_total, g, nullptr, nullptr, nullptr, k, 1, max_iter, tol, seed, nullptr, d_components, h_var,
-                  h_var_ratio, h_mean, info, d_stats, d_gram, d_proj, d_shift, h_l);
+  SB2_CHECK_ARG(ctx && d_stats && d_gram && d_components && h_var && h_var_ratio && h_mean && d_proj && d_shift && h_l,
+                "null pointer");
+  PcaWork w{};
+  SB2_TRY(init_work(ctx, 0, n_total, g, k, 1, w));
+  ScratchScope scr(ctx);
+  SB2_TRY(gene_moments(w, d_stats, h_mean));
+  SB2_TRY(alloc_scratch(w, scr));
+  SB2_CUDA(cudaMemcpyAsync(w.d_mu, h_mean, sizeof(double) * g, cudaMemcpyHostToDevice, w.st));
+  SB2_TRY(gram_operator(w, scr, d_gram, false));
+  SB2_TRY(subspace_iteration(w, scr, k, max_iter, tol, seed));
+  SB2_TRY(projection_operator(w, scr, k, d_components));
+  SB2_CUDA(cudaMemcpyAsync(d_proj, w.d_Bf, sizeof(float) * (size_t)g * w.l, cudaMemcpyDeviceToDevice, w.st));
+  SB2_CUDA(cudaMemcpyAsync(d_shift, w.d_shift, sizeof(float) * w.l, cudaMemcpyDeviceToDevice, w.st));
+  *h_l = w.l;
+  centred_variance(w, k, h_var, h_var_ratio);
+  return report(w, info);
 }
 int32_t sb2_pca_stream_project_f32(sb2_ctx* ctx, int64_t n_chunk, int32_t g, const int64_t* d_indptr,
                                    const int32_t* d_indices, const float* d_data, int32_t k, int32_t l, const float* d_proj,

@@ -68,6 +68,25 @@ def test_pca_matches_reference(synth_small, solver, tol):
     np.testing.assert_allclose(comp @ comp.T, np.eye(k), atol=1e-5)
 
 
+@pytest.mark.parametrize("solver", [1, 0])
+def test_pca_wide_block_matches_fp64(solver):
+    # n_comps between 57 and 120 iterates a 128-wide block, whose Rayleigh-Ritz step is solved on the host; a latent
+    # dimension well above n_comps keeps the spectrum gapped past the cut
+    x, _ = synth_scipy(6000, 800, n_clusters=12, r=160)
+    k = 80
+    out = _ops.pca_csr(x, k, solver=solver)
+    truth = opca.pca_gram_f64(x, k)
+    assert out["converged"]
+    e64 = _rel_err(out["X_pca"], truth["X_pca"])
+    assert e64.max() < 1e-4, (e64.max(), truth["gaps"].min())
+    np.testing.assert_allclose(out["variance"], truth["variance"], rtol=1e-5)
+    np.testing.assert_allclose(out["variance_ratio"], truth["variance_ratio"], rtol=1e-5)
+    # svd_flip(u_based_decision=False) signs: the components match the fp64 truth as they are, not only up to sign
+    comp = out["components"]
+    assert (comp[np.arange(k), np.abs(comp).argmax(axis=1)] > 0).all()
+    np.testing.assert_allclose(comp, truth["components"], atol=2e-4)
+
+
 def test_pca_anndata_writeback_and_mask(synth_small):
     x, _ = synth_small
     x = x[:1500]
