@@ -225,6 +225,27 @@ int32_t sb2_log1p_f32(sb2_ctx* ctx, int64_t nnz, float* d_data, double base);
 int32_t sb2_csr_col_sums_f32(sb2_ctx* ctx, int64_t nnz, int32_t g, const int32_t* d_indices, const float* d_data,
                              int32_t apply_expm1, double log_scale, double* d_sum, double* d_sumsq);
 
+/* ---- quality control and filtering in front of normalize_total (csrc/qc.cu) ----
+ * sb2_csr_qc_rows_f32    <- describe_obs + top_segment_proportions_sparse_csr (src/scanpy/preprocessing/_qc.py:41-129,
+ *                           :430-457) and the per-cell numbers of filter_cells (src/scanpy/preprocessing/_simple.py:53-196).
+ *                           Per row: d_count int64 = #(data != 0), or #(data > 0) with positive_only; d_total fp64 = sum
+ *                           of the stored values; d_qc_total fp64 [n x n_qc] = the sum over the genes whose bit b is set
+ *                           in d_qc_bits[col] (n_qc <= 32; NULL when n_qc == 0); d_top fp64 [n x n_ns] = the sum of the
+ *                           h_ns[i] largest non-zero stored values, padded with zeros up to max(h_ns) as the reference's
+ *                           sparse branch does.  h_ns is a HOST array, sorted ascending, every entry in [1, g].  The top
+ *                           sums are exact selections with a fixed-order fp64 prefix sum: they depend only on the
+ *                           multiset of non-zero values in the row.  max(h_ns) beyond the shared-memory candidate
+ *                           capacity (32768 on sm_90) is an error when some row has more stored values than that.
+ * sb2_csr_col_counts_f32 <- describe_var's axis_nnz (_qc.py:178-180) and filter_genes' `data > 0` count (_simple.py:
+ *                           284-286): d_counts int64 [g] = #(data != 0) (or > 0) per column, overwritten.  The per-gene
+ *                           totals are sb2_csr_col_sums_f32 with apply_expm1 = 0. */
+int32_t sb2_csr_qc_rows_f32(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_indptr, const int32_t* d_indices,
+                            const float* d_data, int32_t positive_only, const uint32_t* d_qc_bits, int32_t n_qc,
+                            const int32_t* h_ns, int32_t n_ns, int64_t* d_count, double* d_total, double* d_qc_total,
+                            double* d_top);
+int32_t sb2_csr_col_counts_f32(sb2_ctx* ctx, int64_t nnz, int32_t g, const int32_t* d_indices, const float* d_data,
+                               int32_t positive_only, int64_t* d_counts);
+
 
 /* ---- extreme eigenpairs of diag(s) A diag(s), A symmetric fp32 CSR (csrc/eigs.cu: thick-restart Lanczos, fp64) ----
  * Replaces `scipy.sparse.linalg.eigsh(matrix.astype(float64), k=n_comps, which='LM', v0=...)` in

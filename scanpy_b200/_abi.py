@@ -119,6 +119,9 @@ SIGNATURES = {
     "sb2_log1p_f32": (c_int32, [c_void_p, c_int64, c_void_p, c_double]),
     "sb2_csr_col_sums_f32": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_int32, c_double, c_void_p,
                                        c_void_p]),
+    "sb2_csr_qc_rows_f32": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_int32,
+                                      c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "sb2_csr_col_counts_f32": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_int32, c_void_p]),
 }
 
 _lib = None

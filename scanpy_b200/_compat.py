@@ -2,7 +2,8 @@
 
 * `MiniAnnData` — a duck-typed stand-in for `anndata.AnnData` (anndata is not installed in the build
   image).  The public functions only use `.X .obs .var .obsm .varm .obsp .uns .n_obs .n_vars
-  .shape .is_view .copy()` and `adata[:, mask]`, so a real AnnData works unchanged.
+  .shape .is_view .copy()`, `adata[:, mask]` and the in-place subsetting the filters call
+  (`_inplace_subset_obs` / `_inplace_subset_var`), so a real AnnData works unchanged.
 * `settings` — the two constants the path reads (`N_PCS`, `n_jobs`; src/scanpy/_settings/__init__.py:83,132)
   plus verbosity-free logging with the reference's message texts (src/scanpy/logging.py:100-131).
 * `accepts_legacy_random_state` — the `random_state=` <-> `rng=` shim of
@@ -117,6 +118,23 @@ class MiniAnnData:
         return MiniAnnData(self.X.copy(), self.obs.copy(), self.var.copy(),
                            {k: v.copy() for k, v in self.obsm.items()}, {k: v.copy() for k, v in self.varm.items()},
                            {k: v.copy() for k, v in self.obsp.items()}, copy.deepcopy(self.uns))
+
+    def _inplace_subset_obs(self, mask):
+        """Keep the cells selected by `mask` (boolean or integer index): X, obs, obsm rows, obsp on both axes, layers."""
+        idx = np.asarray(mask)
+        self.X = self.X[idx]
+        self.obs = self.obs.iloc[idx]
+        self.obsm = _AxisArrays({k: v.iloc[idx] if hasattr(v, "iloc") else v[idx] for k, v in self.obsm.items()})
+        self.obsp = _AxisArrays({k: v[idx][:, idx] for k, v in self.obsp.items()})
+        self.layers = {k: v[idx] for k, v in self.layers.items()}
+
+    def _inplace_subset_var(self, mask):
+        """Keep the genes selected by `mask` (boolean or integer index): X, var, varm rows, layers."""
+        idx = np.asarray(mask)
+        self.X = self.X[:, idx]
+        self.var = self.var.iloc[idx]
+        self.varm = _AxisArrays({k: v.iloc[idx] if hasattr(v, "iloc") else v[idx] for k, v in self.varm.items()})
+        self.layers = {k: v[:, idx] for k, v in self.layers.items()}
 
     def __getitem__(self, idx):
         if not (isinstance(idx, tuple) and len(idx) == 2 and isinstance(idx[0], slice) and idx[0] == slice(None)):
