@@ -246,6 +246,33 @@ int32_t sb2_csr_qc_rows_f32(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d
 int32_t sb2_csr_col_counts_f32(sb2_ctx* ctx, int64_t nnz, int32_t g, const int32_t* d_indices, const float* d_data,
                                int32_t positive_only, int64_t* d_counts);
 
+/* ---- sc.pp.regress_out (src/scanpy/preprocessing/_simple.py:468-681; csrc/regress.cu) ----
+ * X is a block of `rows` rows given either dense (d_x, row-major [rows x g]) or as CSR arrays (d_indptr pointing at the
+ * block's first row, entry offsets absolute; column indices sorted within each row, no duplicates; d_x NULL), with
+ * float32 (is_f64 = 0) or float64 values.
+ * sb2_regress_col_sums  <- `regressor.T @ data` of numpy_regress_out and the per-category means of
+ *                          _create_regressor_categorical.  Weighted (d_w != NULL, fp64 [rows x p], p <= 32): d_acc[k*g+j]
+ *                          += sum_i w[i,k] x[i,j].  Grouped (d_w == NULL): d_acc[c*g+j] += sum of x[i,j] over the rows
+ *                          with d_group[i] == c < n_groups; d_order lists the block's rows sorted by (i / TILE, group, i).
+ *                          Also folds the per-gene min / max into d_min / d_max and sets d_nan[j] if column j holds a NaN
+ *                          (implicit CSR zeros count as 0).  fp64 sums in a fixed order over TILE-row subtiles: calling it
+ *                          over consecutive blocks whose lengths, except the last, are multiples of TILE gives the same
+ *                          bits as one call over all rows.
+ * sb2_regress_residual  <- `data[i] -= regressor[i] @ coeff` / the GLM residuals: d_out[i*g+j] = x[i,j] - fit[i,j], in fp64
+ *                          rounded once to float32 (out_f64 = 0, float32 X only) or float64, fit = sum_k w[i,k] coef[k*g+j]
+ *                          (d_w != NULL) or d_b0[j] + d_b1[j] * d_means[c*g+j] with c = d_code[i] (d_b0[j] for c < 0); genes
+ *                          with d_pass[j] != 0 (d_pass may be NULL) are copied unchanged. */
+#define SB2_REGRESS_TILE_ROWS 1024
+int32_t sb2_regress_col_sums(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f64, const void* d_x,
+                             const int64_t* d_indptr, const int32_t* d_indices, const void* d_data, const double* d_w,
+                             int32_t p, const int32_t* d_group, const int32_t* d_order, int32_t n_groups, double* d_acc,
+                             double* d_min, double* d_max, int32_t* d_nan);
+int32_t sb2_regress_residual(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f64, const void* d_x,
+                             const int64_t* d_indptr, const int32_t* d_indices, const void* d_data, const double* d_w,
+                             int32_t p, const double* d_coef, const int32_t* d_code, const double* d_means,
+                             const double* d_b0, const double* d_b1, const uint8_t* d_pass, int32_t out_f64,
+                             void* d_out);
+
 
 /* ---- extreme eigenpairs of diag(s) A diag(s), A symmetric fp32 CSR (csrc/eigs.cu: thick-restart Lanczos, fp64) ----
  * Replaces `scipy.sparse.linalg.eigsh(matrix.astype(float64), k=n_comps, which='LM', v0=...)` in

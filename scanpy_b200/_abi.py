@@ -122,6 +122,12 @@ SIGNATURES = {
     "sb2_csr_qc_rows_f32": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_int32,
                                       c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
     "sb2_csr_col_counts_f32": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_int32, c_void_p]),
+    "sb2_regress_col_sums": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p,
+                                       c_void_p]),
+    "sb2_regress_residual": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_int32, c_void_p]),
 }
 
 _lib = None

@@ -115,9 +115,11 @@ class MiniAnnData:
     def copy(self):
         import copy
 
-        return MiniAnnData(self.X.copy(), self.obs.copy(), self.var.copy(),
-                           {k: v.copy() for k, v in self.obsm.items()}, {k: v.copy() for k, v in self.varm.items()},
-                           {k: v.copy() for k, v in self.obsp.items()}, copy.deepcopy(self.uns))
+        new = MiniAnnData(self.X.copy(), self.obs.copy(), self.var.copy(),
+                          {k: v.copy() for k, v in self.obsm.items()}, {k: v.copy() for k, v in self.varm.items()},
+                          {k: v.copy() for k, v in self.obsp.items()}, copy.deepcopy(self.uns))
+        new.layers = {k: v.copy() for k, v in self.layers.items()}
+        return new
 
     def _inplace_subset_obs(self, mask):
         """Keep the cells selected by `mask` (boolean or integer index): X, obs, obsm rows, obsp on both axes, layers."""

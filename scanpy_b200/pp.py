@@ -17,6 +17,7 @@ from scipy import sparse
 from . import _ops
 from ._preprocess import highly_variable_genes, log1p, normalize_total, scale  # noqa: F401  (SURVEY 8f row f2)
 from ._qc import calculate_qc_metrics, filter_cells, filter_genes  # noqa: F401
+from ._regress import regress_out  # noqa: F401
 from ._compat import (MiniAnnData, accepts_legacy_random_state, as_csr_f32, is_anndata_like, log_done, log_start,
                       meta_random_state, seed_from_rng, settings, warn)
 
