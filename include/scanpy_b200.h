@@ -273,6 +273,34 @@ int32_t sb2_regress_residual(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f
                              const double* d_b0, const double* d_b1, const uint8_t* d_pass, int32_t out_f64,
                              void* d_out);
 
+/* ---- sc.experimental.pp analytic Pearson residuals (src/scanpy/experimental/pp/_highly_variable_genes.py:35-287,
+ * _normalization.py:36-75; csrc/pearson.cu) ----
+ * X is a block of `rows` rows as for regress_out: dense (d_x) or CSR arrays (d_indptr pointing at the block's first row,
+ * entry offsets absolute; sorted column indices, no duplicates), float32 (is_f64 = 0) or float64 values.  The residual
+ * of x[i,j] is clip((x - mu) / sqrt(mu + mu*mu/theta)) with mu = gene[j] * cell[i] / total, in fp64; clip keeps NaN;
+ * theta may be +inf.
+ * sb2_pearson_row_sums       <- `x.sum(axis=1)`: d_out[i] = fp64 total of row i, in a fixed order.
+ * sb2_pearson_residual_var   <- _calculate_res_sparse / _calculate_res_dense for one batch.  Row k of the call is X row
+ *                               d_order[k] (d_order NULL: row k of the block; with CSR, d_indptr then indexes d_order's
+ *                               rows), d_cell[k] its cell total.  Merges into d_acc fp64 [4 x g] (zeroed before the first
+ *                               call of a batch): row 0 the count, 1 the mean residual, 2 the sum of squared deviations
+ *                               (the variance is M2 / count), 3 Σx².  Blocks of one batch must be consecutive, and all but
+ *                               the last a multiple of SB2_PEARSON_TILE_ROWS rows: the result then has the same bits as
+ *                               one call over the batch.
+ * sb2_pearson_residuals      <- _pearson_residuals: d_out[i*g+j] = the residual, rounded once to float32 (out_f64 = 0,
+ *                               float32 X only) or float64; d_cell[i] is row i's total. */
+#define SB2_PEARSON_TILE_ROWS 1024
+int32_t sb2_pearson_row_sums(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f64, const void* d_x,
+                             const int64_t* d_indptr, const void* d_data, double* d_out);
+int32_t sb2_pearson_residual_var(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f64, const void* d_x,
+                                 const int64_t* d_indptr, const int32_t* d_indices, const void* d_data,
+                                 const int64_t* d_order, const double* d_gene, const double* d_cell, double total,
+                                 double clip, double theta, double* d_acc);
+int32_t sb2_pearson_residuals(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f64, const void* d_x,
+                              const int64_t* d_indptr, const int32_t* d_indices, const void* d_data,
+                              const double* d_gene, const double* d_cell, double total, double clip, double theta,
+                              int32_t out_f64, void* d_out);
+
 
 /* ---- extreme eigenpairs of diag(s) A diag(s), A symmetric fp32 CSR (csrc/eigs.cu: thick-restart Lanczos, fp64) ----
  * Replaces `scipy.sparse.linalg.eigsh(matrix.astype(float64), k=n_comps, which='LM', v0=...)` in

@@ -128,6 +128,11 @@ SIGNATURES = {
     "sb2_regress_residual": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
                                        c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                        c_int32, c_void_p]),
+    "sb2_pearson_row_sums": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "sb2_pearson_residual_var": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, c_double, c_double, c_double, c_void_p]),
+    "sb2_pearson_residuals": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, c_double, c_double, c_double, c_int32, c_void_p]),
 }
 
 _lib = None

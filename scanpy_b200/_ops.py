@@ -111,6 +111,33 @@ def csr_to_device(x):
     return _to_device(indptr), _to_device(indices), _to_device(data)
 
 
+class DeviceX:
+    """X on the device by row blocks, for the entry points that take a dense block or CSR arrays of float32 or float64
+    values (regress_out, the Pearson residuals): a CSR uploaded once (sorted indices, no duplicates), or a dense array
+    uploaded one block at a time.  `block(r0, r1)` -> (d_x, d_indptr, d_indices, d_data)."""
+
+    def __init__(self, x, dtype: np.dtype):
+        from scipy import sparse
+
+        self.is_f64 = int(dtype == np.float64)
+        if sparse.issparse(x):
+            x = x.tocsr()
+            if not x.has_canonical_format:
+                x = x.copy()
+                x.sum_duplicates()
+            self.indptr = _to_device(np.asarray(x.indptr, dtype=np.int64))
+            self.indices = _to_device(np.asarray(x.indices, dtype=np.int32))
+            self.data = _to_device(np.asarray(x.data, dtype=dtype))
+            self.dense = None
+        else:
+            self.dense, self.dtype = x, dtype
+
+    def block(self, r0: int, r1: int):
+        if self.dense is None:
+            return None, self.indptr[r0:], self.indices, self.data
+        return _to_device(np.ascontiguousarray(self.dense[r0:r1], dtype=self.dtype)), None, None, None
+
+
 # ------------------------------------------------------------------------------------------ PCA
 def _pca_call(entry, ctx, args, n_rows, g: int, n_comps: int, *, mean: bool = True, extra=()):
     """`entry(ctx.handle, *args, [X_pca,] components, variance, variance_ratio, [mean,] *extra, &info)` on fresh outputs ->

@@ -48,28 +48,7 @@ def _is_categorical(col: pd.Series) -> bool:
     return isinstance(col.dtype, pd.CategoricalDtype) or col.dtype == object or pd.api.types.is_string_dtype(col.dtype)
 
 
-class _DeviceX:
-    """X on the device by row blocks: a CSR uploaded once (sorted indices, no duplicates), or a dense array uploaded one
-    block at a time.  `block(r0, r1)` -> (d_x, d_indptr, d_indices, d_data) for the entry points."""
-
-    def __init__(self, x, dtype: np.dtype):
-        self.is_f64 = int(dtype == np.float64)
-        if sparse.issparse(x):
-            x = x.tocsr()
-            if not x.has_canonical_format:
-                x = x.copy()
-                x.sum_duplicates()
-            self.indptr = _ops._to_device(np.asarray(x.indptr, dtype=np.int64))
-            self.indices = _ops._to_device(np.asarray(x.indices, dtype=np.int32))
-            self.data = _ops._to_device(np.asarray(x.data, dtype=dtype))
-            self.dense = None
-        else:
-            self.dense, self.dtype = x, dtype
-
-    def block(self, r0: int, r1: int):
-        if self.dense is None:
-            return None, self.indptr[r0:], self.indices, self.data
-        return _ops._to_device(np.ascontiguousarray(self.dense[r0:r1], dtype=self.dtype)), None, None, None
+_DeviceX = _ops.DeviceX
 
 
 def _col_sums(dx: _DeviceX, n: int, g: int, *, w=None, group=None, n_groups: int = 0):

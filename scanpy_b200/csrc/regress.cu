@@ -14,49 +14,20 @@
 // fit = sum_k W[i, k] B[k, j] or b0[j] + b1[j] * means[code_i, j] (b0[j] for code -1); genes flagged in `pass` are
 // copied.  Writes the dense row block; HBM-bound.
 //
-// A CSR input is read in place in both passes: every CTA binary-searches its column slab in each row (indices must be
-// sorted, no duplicates) and scatters the slab's stored values into a zeroed shared-memory tile, so implicit zeros
-// enter the sums and the min / max as zeros.
+// A CSR input is read in place in both passes (slab.cuh: `stage_csr`), so implicit zeros enter the sums and the min /
+// max as zeros.
 #include <math.h>
 
 #include "common.cuh"
+#include "slab.cuh"
 
 namespace {
 
-constexpr int RG_THREADS = 256;  // one column per thread: 256-column slabs
-constexpr int RG_ROWS = 16;      // rows staged per step
+constexpr int RG_THREADS = SLAB_THREADS;
+constexpr int RG_ROWS = SLAB_ROWS;
 constexpr int RG_TILE = SB2_REGRESS_TILE_ROWS;
 constexpr int RG_MAXP = 32;
 static_assert(RG_TILE % RG_ROWS == 0, "subtile");
-
-// The slab [c0, c1) of the m rows rid[0..m) of a CSR, scattered into tile[r][col - c0]; tile must be zero on entry.
-// Thread r < m has written rid[r] before the call; the caller clears what it reads.
-template <typename T>
-__device__ __forceinline__ void stage_csr(const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
-                                          const T* __restrict__ data, const int64_t* rid, int m, int c0, int c1,
-                                          T (*tile)[RG_THREADS], int64_t* lo, int64_t* hi) {
-  if ((int)threadIdx.x < m) {
-    const int64_t r = rid[threadIdx.x];
-    const int64_t e1 = indptr[r + 1];
-    int64_t a = indptr[r], b = e1;
-    while (a < b) {
-      const int64_t mid = (a + b) >> 1;
-      if (indices[mid] < c0) a = mid + 1; else b = mid;
-    }
-    lo[threadIdx.x] = a;
-    b = e1;
-    while (a < b) {
-      const int64_t mid = (a + b) >> 1;
-      if (indices[mid] < c1) a = mid + 1; else b = mid;
-    }
-    hi[threadIdx.x] = a;
-  }
-  __syncthreads();
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  for (int r = warp; r < m; r += RG_THREADS / 32)
-    for (int64_t e = lo[r] + lane; e < hi[r]; e += 32) tile[r][indices[e] - c0] = data[e];
-  __syncthreads();
-}
 
 // grid (subtiles, slabs).  Weighted (w != NULL): part[sub][k][j], k < p.  Categorical: part[sub][group][j], the groups a
 // subtile lacks stay as the caller zeroed them; `order` lists each subtile's rows sorted by (group, row).
