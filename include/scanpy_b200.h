@@ -190,7 +190,9 @@ int32_t sb2_knn_connectivities_f64(sb2_ctx* ctx, int64_t n, int32_t k, const int
 
 /* ---- Leiden on a symmetric weighted CSR graph ------------------------------------------------
  * n_iterations < 0: iterate until a whole pass moves nothing.  Output membership int32[n]
- * renumbered by decreasing community size; *h_modularity at the given resolution. */
+ * renumbered by decreasing community size; *h_modularity at the given resolution.  Weights must be finite and
+ * non-negative (SB2_E_BADARG otherwise); results do not change when every weight is multiplied by a power of two.
+ * sb2_modularity_csr_f32: d_membership ids in [0, n). */
 int32_t sb2_leiden_csr_f32(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, const int32_t* d_indices,
                            const float* d_weights, double resolution, int32_t n_iterations, uint64_t seed,
                            int32_t* d_membership, double* h_modularity, int32_t* h_n_comms, sb2_leiden_info* info);

@@ -462,10 +462,18 @@ def louvain(adj, *, resolution: float = 1.0, seed: int = 0, ctx=None):
 
 
 def modularity(adj, membership, *, resolution: float = 1.0, ctx=None) -> float:
-    ctx = ctx or _abi.default_context()
+    """Modularity of `membership` (any non-negative integer ids, gaps allowed) on a symmetric scipy CSR adjacency."""
     adj = adj.tocsr()
+    membership = np.asarray(membership).ravel()
+    if membership.shape[0] != adj.shape[0]:
+        raise ValueError(f"membership has {membership.shape[0]} entries for a graph of {adj.shape[0]} vertices")
+    if membership.size and membership.min() < 0:
+        raise ValueError("membership ids must be non-negative (a negative code marks a missing label)")
+    # sb2_modularity_csr_f32 takes ids in [0, n): compact them (unused ids - e.g. unused categories - do not change Q)
+    _, codes = np.unique(membership, return_inverse=True)
+    ctx = ctx or _abi.default_context()
     d_indptr, d_indices, d_w = csr_to_device(adj)
-    d_m = _to_device(np.asarray(membership, dtype=np.int32))
+    d_m = _to_device(codes.astype(np.int32))
     q = c_double()
     check(ctx.lib.sb2_modularity_csr_f32(ctx.handle, adj.shape[0], ptr(d_indptr), ptr(d_indices), ptr(d_w),
                                          float(resolution), ptr(d_m), byref(q)))

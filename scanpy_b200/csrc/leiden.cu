@@ -18,8 +18,12 @@
 //   agg_* kernels         refined communities become super-vertices: per-super-vertex open-addressing
 //                         hash slices (capacity = sum of member degrees) accumulate the edge weights.
 // Determinism: moves are decided against a snapshot and applied in a separate kernel; every
-// accumulated quantity (edge weights, strengths K_c) is a 2^-32 fixed-point int64, so atomic order
+// accumulated quantity (edge weights, strengths K_c) is a fixed-point int64, so atomic order
 // cannot change any sum; ties break towards the smaller community id.  Same seed => same labels.
+// Fixed point: one unit is 2^-e of the input weight, e = 32 - ceil(log2(max arc weight)) (lower by one bit per doubling
+// beyond 2^30 arcs), so the largest arc is <= 2^32 units and the total < 2^62.  The objective is invariant under a
+// uniform weight scale and the scale is a power of two, so w and w * 2^k give bit-identical runs; UMAP connectivities
+// (max weight 1) get e = 32.  NaN, infinite or negative weights are rejected (SB2_E_BADARG).
 // HBM-bound integer/gather work; per local-move sweep ~ 12*E (idx + weight) + 4*E (community gather) B.
 #include <math.h>
 #include <string.h>
@@ -32,7 +36,6 @@
 namespace {
 
 typedef unsigned long long u64;
-constexpr double FX = 4294967296.0;  // 2^32 fixed-point scale
 
 struct Level {
   int32_t n;
@@ -47,9 +50,38 @@ __host__ __device__ __forceinline__ uint32_t mix32(uint32_t x) {
   return x;
 }
 
-__global__ void to_fixed_kernel(const float* __restrict__ w, int64_t n, int64_t* __restrict__ out) {
+// One read of the arc weights: scan[0] = bit pattern of the largest weight (non-negative floats order like their bits as
+// int32), scan[1] = 1 if some weight is NaN, infinite or negative (-0.0 counts as 0).
+__global__ void weight_scan_kernel(const float* __restrict__ w, int64_t n, int32_t* __restrict__ scan) {
+  int32_t mx = 0, bad = 0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const float x = w[i];
+    if (!(x >= 0.0f) || isinf(x)) bad = 1;
+    else mx = max(mx, __float_as_int(x));
+  }
+  mx = __reduce_max_sync(0xffffffffu, mx);
+  bad = __reduce_or_sync(0xffffffffu, bad);
+  if ((threadIdx.x & 31) == 0) {
+    if (mx) atomicMax(&scan[0], mx);
+    if (bad) atomicOr(&scan[1], 1);
+  }
+}
+// ceil(log2(x)) of a positive finite float given by its bits (normal or subnormal)
+__device__ __forceinline__ int ceil_log2_f32(int32_t bits) {
+  const int32_t be = bits >> 23, man = bits & 0x7FFFFF;
+  if (be == 0) return -149 + (32 - __clz(man - 1));   // subnormal: man * 2^-149
+  return be - 127 + (man != 0);
+}
+// Fixed point with a per-graph power-of-two scale 2^e, e = 32 - ceil(log2(max w)) - extra_shift: the largest arc becomes
+// at most 2^32 units, so a total of up to 2^30 arcs stays below 2^62 (extra_shift lowers e for more arcs).  A power of two
+// keeps the conversion exact under power-of-two rescaling of the input: w * 2^k gives the same int64 weights.
+__global__ void to_fixed_kernel(const float* __restrict__ w, int64_t n, const int32_t* __restrict__ scan, int extra_shift,
+                                int64_t* __restrict__ out) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = llrint((double)w[i] * FX);
+  if (i >= n) return;
+  const int32_t mx = scan[0];
+  const int e = (mx > 0 ? 32 - ceil_log2_f32(mx) : 32) - extra_shift;
+  out[i] = llrint(scalbn((double)w[i], e));   // (a flagged graph is rejected before these values are used)
 }
 __global__ void strength_kernel(int32_t n, const int64_t* __restrict__ indptr, const int64_t* __restrict__ w,
                                 int64_t* __restrict__ k, u64* __restrict__ total) {
@@ -140,7 +172,7 @@ decide_kernel(Level L, const int32_t* __restrict__ wl, int32_t w_begin, int32_t 
       }
     }
     // lanes that look at the same community form a group (MATCH.ANY); the group's arc weights - non-negative
-    // 2^-32 fixed point, < 2^63 in total - are summed exactly with three 24-bit-limb warp reductions (REDUX) instead
+    // fixed point, <= 2^32 each - are summed exactly with three 24-bit-limb warp reductions (REDUX) instead
     // of 32 rounds of shuffles
     const unsigned grp = __match_any_sync(0xffffffffu, c);
     const bool leader = (__ffs(grp) - 1) == lane;
@@ -719,19 +751,32 @@ static int32_t prepare_level0(sb2_ctx* ctx, ScratchScope& scr, int64_t n, const 
   *nnz_out = nnz;
   SB2_TRY(scr.alloc(wfx, (size_t)nnz));
   SB2_TRY(scr.alloc(kfx, (size_t)n));
-  u64* tot;
+  u64* tot;   // [0] total, [1] the weight scan (two int32)
   SB2_TRY(scr.alloc(&tot, 2));
+  int32_t* scan = (int32_t*)(tot + 1);
   SB2_CUDA(cudaMemsetAsync(tot, 0, 16, st));
+  // every fixed-point arc is <= 2^32 units; beyond 2^30 arcs the scale drops by the missing bits so that the total
+  // stays below 2^62
+  int extra_shift = 0;
+  while ((nnz >> extra_shift) > ((int64_t)1 << 30)) ++extra_shift;
   if (nnz > 0) {
-    to_fixed_kernel<<<gridt(nnz), 256, 0, st>>>(d_weights, nnz, *wfx);
+    weight_scan_kernel<<<(unsigned)std::min<int64_t>(gridt(nnz), 1024), 256, 0, st>>>(d_weights, nnz, scan);
+    SB2_LAUNCH_CHECK(ctx);
+    to_fixed_kernel<<<gridt(nnz), 256, 0, st>>>(d_weights, nnz, scan, extra_shift, *wfx);
     SB2_LAUNCH_CHECK(ctx);
   }
   strength_kernel<<<gridt(n), 256, 0, st>>>((int32_t)n, d_indptr, *wfx, *kfx, tot);
   SB2_LAUNCH_CHECK(ctx);
-  u64 ht = 0;
-  SB2_CUDA(cudaMemcpyAsync(&ht, tot, sizeof(u64), cudaMemcpyDeviceToHost, st));
+  u64 ht[2] = {0, 0};
+  SB2_CUDA(cudaMemcpyAsync(ht, tot, sizeof(ht), cudaMemcpyDeviceToHost, st));
   SB2_CUDA(cudaStreamSynchronize(st));
-  *total = (double)(long long)ht;
+  int32_t hscan[2];
+  memcpy(hscan, &ht[1], sizeof(hscan));
+  if (hscan[1]) {
+    sb2_set_error("bad argument: edge weights must be finite and non-negative (found NaN, inf or a negative weight)");
+    return SB2_E_BADARG;
+  }
+  *total = (double)(long long)ht[0];
   return SB2_OK;
 }
 

@@ -51,4 +51,5 @@ def modularity(adata_or_connectivities, /, labels="leiden", *, neighbors_key: st
             raise NotImplementedError("directed modularity of a non-symmetric adjacency is not implemented in scanpy_b200")
     if adj.dtype != np.float32:
         adj = adj.astype(np.float32)
-    return float(_ops.modularity(adj, np.asarray(_codes(labels), dtype=np.int32), resolution=1.0))
+    # a missing label has code -1, which _ops.modularity rejects (igraph rejects a negative membership too)
+    return float(_ops.modularity(adj, np.asarray(_codes(labels)), resolution=1.0))

@@ -62,6 +62,22 @@ def _restrict_adjacency(adata, restrict_key: str, *, restrict_categories: Sequen
     return adjacency, restrict_indices
 
 
+def _clustering_graph(adjacency, *, use_weights: bool):
+    """The float32 CSR graph tl.leiden / tl.louvain cluster.  The reference builds its igraph from `adjacency.nonzero()`
+    (_utils/__init__.py:292-298): a stored zero is not an edge, so explicit zeros are dropped (on a copy) before
+    `use_weights=False` turns every stored arc into weight 1.  A graph without stored zeros is passed on as it is."""
+    adj = adjacency.tocsr()
+    if adj.dtype != np.float32:
+        adj = adj.astype(np.float32)
+    if np.count_nonzero(adj.data) < adj.data.size:
+        adj = adj.copy()
+        adj.eliminate_zeros()
+    if not use_weights:
+        adj = adj.copy()
+        adj.data[:] = 1.0
+    return adj
+
+
 def _rename_groups(adata, restrict_key, *, restrict_categories, restrict_indices, groups):
     all_groups = adata.obs[restrict_key].astype("U").copy()
     prefix = f"{'-'.join(restrict_categories)},"
@@ -88,12 +104,7 @@ def leiden(adata, resolution: float = 1, *, restrict_to=None, rng=None, key_adde
         restrict_key, restrict_categories = restrict_to
         adjacency, restrict_indices = _restrict_adjacency(adata, restrict_key, restrict_categories=restrict_categories,
                                                           adjacency=adjacency)
-    adj = adjacency.tocsr()
-    if adj.dtype != np.float32:
-        adj = adj.astype(np.float32)
-    if not use_weights:
-        adj = adj.copy()
-        adj.data[:] = 1.0
+    adj = _clustering_graph(adjacency, use_weights=use_weights)
     groups, modularity, _info = _ops.leiden(adj, resolution=1.0 if resolution is None else float(resolution),
                                             n_iterations=n_iterations, seed=seed_from_rng(rng))
     if restrict_to is not None:
@@ -147,12 +158,7 @@ def louvain(adata, resolution: float | None = None, *, random_state=0, restrict_
                                                           adjacency=adjacency)
     if flavor == "igraph" and resolution is not None:
         warn('`resolution` parameter has no effect for flavor "igraph"')
-    adj = adjacency.tocsr()
-    if adj.dtype != np.float32:
-        adj = adj.astype(np.float32)
-    if not use_weights:
-        adj = adj.copy()
-        adj.data[:] = 1.0
+    adj = _clustering_graph(adjacency, use_weights=use_weights)
     gamma = 1.0 if (resolution is None or flavor == "igraph") else float(resolution)
     # `random_state` is the legacy form here (int | None | RandomState, _louvain.py:53): fold it to the kernels' integer seed
     seed = int(random_state) if isinstance(random_state, (int, np.integer)) else seed_from_rng(LegacyRng(random_state))
