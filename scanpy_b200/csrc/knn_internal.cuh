@@ -12,6 +12,7 @@ struct KnnTc2Shape {
   int kpad;     // padded K axis (terms*d + 3 rounded up to 16*nsplit)
   int terms;
   int est;      // 1: the sweep may start from a sampled threshold
+  int pipe;     // 1: the shape allows the pipelined consumer loop (nsplit == 1, nstage >= 3)
   size_t smem;
 };
 bool knn_tc2_supported(int d);

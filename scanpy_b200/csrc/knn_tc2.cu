@@ -9,25 +9,29 @@
 // with hi = fp16(x), lo = fp16(x - hi) and h0+h1+h2 = -|c|^2/2 (three-way fp16 split); K is padded to a multiple of 16
 // (d = 50: 64 and 160).  knn.cu runs terms = 1 first and re-sweeps the rows it cannot certify with terms = 3.
 //
-// Shape (one CTA per SM, 9 warps):
+// Shape (one CTA per SM, 9 warps, or 12 in the pipelined loop):
 //   CTA = 128 queries x all candidate tiles of 128 points.
 //     warps 0-7   two consumer warpgroups; warpgroup g owns query rows 64g..64g+63 and issues, per tile, the k-steps of
 //                 wgmma.m64n128k16 (A = its 64 query rows, B = the staged candidate tile, both from shared memory, fp32
-//                 accumulators in registers), waits for them, hands the ring stage back and examines the 64 x 128
-//                 scores in registers.  While one warpgroup examines, the other one's MMAs run.  In the accumulator
+//                 accumulators in registers) and examines the 64 x 128 scores in registers.  Pipelined loop (K = 64 and
+//                 K = 160 with whole tiles per ring stage): two accumulator sets, tile c+1's MMAs are issued before
+//                 the warpgroup examines tile c, so each warpgroup's own MMAs run under its scan.  Otherwise: issue,
+//                 wait, hand the stage back, examine (only the other warpgroup's MMAs can overlap).  In the accumulator
 //                 fragment a thread holds two rows and, of each, the 32 columns with (column / 2) % 4 = lane % 4; every
 //                 (row, lane % 4) keeps its OWN register-resident proposal sub-list (16 or 32 scores in groups of 8 with
 //                 group minima; ids write-only to global memory): four disjoint sub-lists per row, no cross-thread
 //                 traffic in the loop.  A point outside all four sub-lists of a row scored at most max(tau_0..tau_3),
 //                 which is what the re-score certificate uses.
 //     warp 8      producer: 1-D cp.async.bulk of pre-arranged candidate images (or K-slices of them) into an mbarrier
-//                 ring that takes the shared memory left after the query image
+//                 ring that takes the shared memory left after the query image (pipelined loop: warps 8-11, so that
+//                 setmaxnreg can hand their registers to the consumers)
 //   Starting threshold: the first n/16 visits sweep every 16th tile and keep the 6 largest chunk maxima per (row,
 //   sub-list); the four sub-lists of a row (four lanes of one warp) are merged by shuffles once and the 6th largest of
 //   the 24 seeds all four (rank ~96 of the row).
 //   Sweep front: CTAs walk the candidate tiles cyclically, starting where the running CTAs currently are (g_knn2_front).
 #include <cuda_fp16.h>
 #include <float.h>
+#include <string.h>
 
 #include "common.cuh"
 #include "knn_internal.cuh"
@@ -43,6 +47,14 @@ constexpr int BAR_BYTES = 1024;    // mbarriers IN FRONT of the operand images
 constexpr int NCONS = 8;           // consumer warps (two warpgroups)
 constexpr int THREADS = (NCONS + 1) * 32;
 constexpr int W_PROD = NCONS;
+// pipelined loop: the producer gets a warpgroup of its own so that setmaxnreg can move registers from it to the
+// consumers (two accumulator sets do not fit the 168 registers a thread gets when 288 or 384 threads share the file)
+constexpr int THREADS_PIPE = (NCONS + 4) * 32;
+constexpr int PROD_REGS = 40, CONS_REGS = 232;
+// k-steps the pipelined loop is compiled for: K = 64 (fp16 operands, d <= 61) and K = 160 (fp16 up to d = 157, split
+// fp16 at d = 50); other K axes take the single-buffer loop
+constexpr int PIPE_NKS0 = 4, PIPE_NKS1 = 10;
+static_assert(128 * PROD_REGS + 256 * CONS_REGS <= 65536 / THREADS_PIPE / 8 * 8 * THREADS_PIPE, "register file");
 constexpr int NSUB = 4;            // sub-lists per query row
 constexpr int EST_R = 6;
 constexpr uint32_t SBO = 128;              // bytes between 8-row groups (core matrices contiguous)
@@ -184,10 +196,13 @@ __device__ __forceinline__ float max8u(const uint32_t* v) {
 // maxima, so the latencies overlap) and one compare.  Rare path: visit the quarters whose
 // maximum beats tau, copy the quarter's eight values aside and pull its maxima out one by one.  The quarter loop is
 // NOT unrolled: one copy of the extraction and insertion code per call site keeps the kernel in the instruction caches.
-template <int NG>
+// stamp(PH_SCAN) / stamp(PH_INSERT) bracket the rare path for the opt-in phase stamps (no-ops when they are off).
+enum { PH_WAIT = 0, PH_MMA, PH_SCAN, PH_INSERT, PH_N };
+template <int NG, class Stamp>
 __device__ __forceinline__ void scan_chunk(SubList<NG>& L, int32_t* __restrict__ id, const uint32_t (&v)[32], int32_t cand0,
-                                           int32_t n_points) {
+                                           int32_t n_points, const Stamp& stamp) {
   const float h0 = max8u(&v[0]), h1 = max8u(&v[8]), h2 = max8u(&v[16]), h3 = max8u(&v[24]);
+  stamp(PH_SCAN);
   if (fmaxf(fmax3(h0, h1, h2), h3) > L.tau) {
 #pragma unroll 1
     for (int q = 0; q < 4; ++q) {
@@ -215,6 +230,7 @@ __device__ __forceinline__ void scan_chunk(SubList<NG>& L, int32_t* __restrict__
       }
     }
   }
+  stamp(PH_INSERT);
 }
 // estimate phase: keep the EST_R largest values seen (sorted descending), branch-free
 template <int LEN>
@@ -239,13 +255,26 @@ __device__ __forceinline__ void est_chunk(float (&est)[LEN], const uint32_t (&v)
 // (resident CTAs): starting a new CTA at the position last published by ANY running CTA lets the spread of the pack
 // grow from wave to wave; re-centring every new CTA on the mean bounds it by the drift of a single lap.
 __device__ unsigned long long g_knn2_front;   // sweep-proper visits of all CTAs of this launch, in units of 16 tiles
-template <int NG>
-__global__ void __launch_bounds__(THREADS, 1)
+// PNKS = 0: single-buffer loop.  Per tile, a warpgroup issues its nks k-steps, waits for all of them, releases the stage
+//   and scans; the only overlap is whatever the other warpgroup's MMAs happen to do meanwhile.  Any nsplit / nstage.
+// PNKS > 0: pipelined loop, nks = PNKS.  Two accumulator sets; tile c+1's MMAs are issued (and run) while the warpgroup
+//   scans tile c, so every warpgroup keeps the tensor pipe fed on its own.  A warpgroup then holds two ring stages at a
+//   time: needs nsplit = 1 and nstage >= 3 (knn_tc2_shape sets KnnTc2Shape::pipe), and 384 threads (THREADS_PIPE,
+//   registers rebalanced).  The k-step count is a template argument because ptxas serialises every wgmma of the kernel
+//   when a loop with a run-time trip count issues them while another group is in flight.
+// STAMPS: lane 0 of warp 0 of each consumer warpgroup adds up clock64() per phase (PH_WAIT on full[s], PH_MMA issue to
+//   end of the wgmma wait, PH_SCAN examination incl. estimate / seeding / release, PH_INSERT the rare path of
+//   scan_chunk) in shared memory and writes stamps[(cta * 2 + warpgroup) * PH_N + phase] at the end.  A template
+//   argument, not a run-time test: even never-taken uniform branches inside the scan cost the single-buffer loop 8 %
+//   (they split the examination into blocks the scheduler cannot interleave).
+template <int NG, int PNKS, bool STAMPS>
+__global__ void __launch_bounds__(PNKS > 0 ? THREADS_PIPE : THREADS, 1)
 knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bimg, int nks, int nsplit, int nstage,
                   int64_t n_btiles, int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points,
-                  float* __restrict__ cand_score, int32_t* __restrict__ cand_idx) {
+                  float* __restrict__ cand_score, int32_t* __restrict__ cand_idx, unsigned long long* __restrict__ stamps) {
+  constexpr bool PIPE = PNKS > 0;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  const uint32_t part_b = (uint32_t)(CN * 16 * 2) * (uint32_t)nks;      // bytes per staged K-slice of a candidate image
+  const uint32_t part_b = (uint32_t)(CN * 16 * 2) * (uint32_t)nks;     // bytes per staged K-slice of a candidate image
   const uint32_t tile_b = part_b * (uint32_t)nsplit;                    // bytes per 128-row image (query or candidate)
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw);
   unsigned char* As = smem_raw + BAR_BYTES;
@@ -254,7 +283,8 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
   uint64_t* empty = bars + MAXST;         // [MAXST] consumer warps -> producer
   uint64_t* afull = bars + 2 * MAXST;     // [1]
   int32_t* start_tile = reinterpret_cast<int32_t*>(bars + 2 * MAXST + 1);
-  static_assert((2 * MAXST + 2) * 8 <= BAR_BYTES, "barrier block");
+  unsigned long long* stamp_sm = reinterpret_cast<unsigned long long*>(bars + 2 * MAXST + 2);  // [2][PH_N + 1]
+  static_assert((2 * MAXST + 2 + 2 * (PH_N + 1)) * 8 <= BAR_BYTES, "barrier block");
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -270,9 +300,10 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
   }
   __syncthreads();
 
-  if (warp == W_PROD) {
+  if (warp >= W_PROD) {
     // ---------------- producer ----------------
-    if (lane == 0) {
+    if constexpr (PIPE) setmaxnreg_dec<PROD_REGS>();
+    if (warp == W_PROD && lane == 0) {
       mbar_expect_tx(afull, tile_b);
       bulk_g2s(As, reinterpret_cast<const unsigned char*>(Aimg) + (size_t)(qtile0 + (int64_t)blockIdx.x) * tile_b, tile_b, afull);
       // visit order: n_est sample tiles (every est_stride-th) for the threshold estimate, then every tile
@@ -296,6 +327,7 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
   }
 
   // ---------------- consumers: thread <-> (two query rows, sub-list lane % 4) ----------------
+  if constexpr (PIPE) setmaxnreg_inc<CONS_REGS>();
   const int g = warp >> 2;                                   // warpgroup: query rows 64g .. 64g+63
   const int sl = lane & 3;                                   // sub-list = column class of the fragment
   const int row0 = 64 * g + 16 * (warp & 3) + (lane >> 2);   // rows row0 and row0 + 8
@@ -319,9 +351,6 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
   static_assert(EST_R <= LS, "estimate aliases the list registers");
 #pragma unroll
   for (int i = 0; i < LS; ++i) { L0.ls[i] = -INFINITY; L1.ls[i] = -INFINITY; }
-  float acc[64];
-#pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
   // descriptors: A = this warpgroup's 64 rows of the query image, B = ring stage 0; one k-step (two 8-column K-chunks)
   // advances the start address by 2 * LBO bytes (the address field counts 16-byte units)
   const uint64_t da0 = wgmma_desc(smem_u32(As) + (uint32_t)g * 8u * SBO, LBO, SBO);
@@ -332,24 +361,23 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
   int32_t ctile = *start_tile;                 // candidate tile of the current sweep visit (cyclic walk)
   int32_t cbase = ctile * CN + 2 * sl;
   const int32_t n_bt = (int32_t)n_btiles;
-  int s = 0;
-  uint32_t ring_phase = 0;
-  mbar_wait(afull, 0);
-  for (int c = 0; c < n_visit; ++c) {
-    for (int p = 0; p < nsplit; ++p) {
-      mbar_wait(&full[s], ring_phase);
-      wgmma_fence();
-      const uint64_t da = da0 + (uint64_t)((uint32_t)(p * nks) * KSTEP16);
-      const uint64_t db = db0 + (uint64_t)((uint32_t)s * part16);
-      for (int j = 0; j < nks; ++j)
-        wgmma_m64n128k16_f16(acc, da + (uint64_t)((uint32_t)j * KSTEP16), db + (uint64_t)((uint32_t)j * KSTEP16), (p | j) != 0);
-      wgmma_commit();
-      wgmma_wait_all();
-      // this warp's reads of the stage are complete: the eighth arrival lets the producer refill it
+
+  // phase stamps (opt-in): no code at all without STAMPS
+  const bool stamp_on = STAMPS && (warp & 3) == 0;
+  unsigned long long* my_st = stamp_sm + g * (PH_N + 1);   // [PH_N] totals, [PH_N] clock of the previous stamp
+  const auto stamp = [&](int ph) {
+    if (stamp_on) {
       __syncwarp();
-      if (lane == 0) mbar_arrive(&empty[s]);
-      if (++s == nstage) { s = 0; ring_phase ^= 1u; }
+      if (lane == 0) {
+        const unsigned long long now = (unsigned long long)clock64();
+        my_st[ph] += now - my_st[PH_N];
+        my_st[PH_N] = now;
+      }
     }
+  };
+
+  // everything a warpgroup does with the scores of visit c once they are in acc
+  const auto examine = [&](const float (&acc)[64], int c) {
     if (c == n_est_i) {
       // start of the sweep proper: seed the sub-lists.  With an estimate phase the four sub-lists of a row (lanes
       // lane ^ 1, ^ 2, ^ 3) are merged: the 6th largest of their 24 chunk maxima sits at about rank 6 * est_stride = 96
@@ -388,12 +416,104 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
       est_chunk(L0.ls, v0);
       est_chunk(L1.ls, v1);
     } else {
-      scan_chunk(L0, id0, v0, cbase, n_points);
-      scan_chunk(L1, id1, v1, cbase, n_points);
+      scan_chunk(L0, id0, v0, cbase, n_points, stamp);
+      scan_chunk(L1, id1, v1, cbase, n_points, stamp);
       if ((c & 15) == 0 && warp == 0 && lane == 0) atomicAdd(&g_knn2_front, 1ull);   // 16 more visits of the pack
       cbase += CN;
       if (++ctile == n_bt) { ctile = 0; cbase = 2 * sl; }
     }
+  };
+
+  mbar_wait(afull, 0);
+  if (stamp_on && lane == 0) {
+    for (int ph = 0; ph < PH_N; ++ph) my_st[ph] = 0ull;
+    my_st[PH_N] = (unsigned long long)clock64();
+  }
+  if constexpr (PIPE) {
+    // steady state per warpgroup: wait full[stage(c+1)], issue tile c+1 into the other accumulator set, wait until
+    // only that group is in flight, release stage(c), examine tile c under tile c+1's MMAs.  The loop is unrolled by
+    // two so that both accumulator sets keep static register indices.
+    float accA[64], accB[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) { accA[i] = 0.0f; accB[i] = 0.0f; }
+    int s_iss = 0, s_rel = 0;     // ring stage of the next tile to issue / of the tile to examine next
+    uint32_t ph_iss = 0;
+    const auto issue = [&](float (&acc)[64]) {
+      mbar_wait(&full[s_iss], ph_iss);
+      stamp(PH_WAIT);
+      wgmma_fence_operand(acc);
+      wgmma_fence();
+      const uint64_t db = db0 + (uint64_t)((uint32_t)s_iss * part16);
+#pragma unroll
+      for (int j = 0; j < PNKS; ++j)
+        wgmma_m64n128k16_f16(acc, da0 + (uint64_t)((uint32_t)j * KSTEP16), db + (uint64_t)((uint32_t)j * KSTEP16), j != 0);
+      wgmma_commit();
+      if (++s_iss == nstage) { s_iss = 0; ph_iss ^= 1u; }
+    };
+    const auto release = [&]() {
+      // this warp's reads of the stage are complete: the eighth arrival lets the producer refill it
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[s_rel]);
+      if (++s_rel == nstage) s_rel = 0;
+    };
+    // tile c is in flight in cur: issue tile c+1 into nxt, examine tile c
+    const auto step = [&](float (&cur)[64], float (&nxt)[64], int c) {
+      issue(nxt);
+      wgmma_wait<1>();     // tile c's group is complete, tile c+1's still runs
+      wgmma_fence_operand(cur);
+      stamp(PH_MMA);
+      release();
+      examine(cur, c);
+      stamp(PH_SCAN);
+    };
+    // the last tile, in flight in cur
+    const auto last = [&](float (&cur)[64], int c) {
+      wgmma_wait<0>();
+      wgmma_fence_operand(cur);
+      stamp(PH_MMA);
+      release();
+      examine(cur, c);
+      stamp(PH_SCAN);
+    };
+    // each exit has its own epilogue: merging the two sets after the loop (or testing "is there a next tile" apart
+    // from the loop exit) makes ptxas see accumulator copies while a group is in flight and serialise every wgmma
+    issue(accA);
+    stamp(PH_MMA);
+    for (int c = 0;; c += 2) {
+      if (c + 1 == n_visit) { last(accA, c); break; }
+      step(accA, accB, c);
+      if (c + 2 == n_visit) { last(accB, c + 1); break; }
+      step(accB, accA, c + 1);
+    }
+  } else {
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+    int s = 0;
+    uint32_t ring_phase = 0;
+    for (int c = 0; c < n_visit; ++c) {
+      for (int p = 0; p < nsplit; ++p) {
+        mbar_wait(&full[s], ring_phase);
+        stamp(PH_WAIT);
+        wgmma_fence();
+        const uint64_t da = da0 + (uint64_t)((uint32_t)(p * nks) * KSTEP16);
+        const uint64_t db = db0 + (uint64_t)((uint32_t)s * part16);
+        for (int j = 0; j < nks; ++j)
+          wgmma_m64n128k16_f16(acc, da + (uint64_t)((uint32_t)j * KSTEP16), db + (uint64_t)((uint32_t)j * KSTEP16), (p | j) != 0);
+        wgmma_commit();
+        wgmma_wait_all();
+        stamp(PH_MMA);
+        // this warp's reads of the stage are complete: the eighth arrival lets the producer refill it
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
+        if (++s == nstage) { s = 0; ring_phase ^= 1u; }
+      }
+      examine(acc, c);
+      stamp(PH_SCAN);
+    }
+  }
+  if (stamp_on && lane == 0) {
+    for (int ph = 0; ph < PH_N; ++ph) stamps[((size_t)blockIdx.x * 2 + g) * PH_N + ph] = my_st[ph];
   }
   if (valid0) {
 #pragma unroll
@@ -423,6 +543,9 @@ bool knn_tc2_shape(const sb2_ctx* ctx, int d, int terms, bool want_estimate, Knn
       int nst = (int)((cap - fixed) / part);
       if (nst > MAXST) nst = MAXST;
       out->nsplit = ns; out->nstage = nst; out->kpad = kp; out->terms = terms; out->est = want_estimate ? 1 : 0;
+      // the pipelined loop holds two stages per warpgroup (the one it examines, the one its MMAs read): whole tiles
+      // per stage, and a third stage so that the producer can run ahead; compiled for K = 64 and K = 160
+      out->pipe = (ns == 1 && nst >= 3 && (kp == 16 * PIPE_NKS0 || kp == 16 * PIPE_NKS1)) ? 1 : 0;
       out->smem = fixed + (size_t)nst * part;
       return true;
     }
@@ -453,15 +576,51 @@ int32_t knn_tc2_build_images(sb2_ctx* ctx, const KnnTc2Shape& sh, const float* d
 }
 
 namespace {
-template <int NG>
-cudaError_t launch2(unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B, int64_t n_tiles,
-                    int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs, int32_t* ci) {
-  cudaError_t e = cudaFuncSetAttribute(knn_sweep2_kernel<NG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
+template <int NG, int PNKS, bool STAMPS>
+cudaError_t launch2s(unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B, int64_t n_tiles,
+                     int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs, int32_t* ci,
+                     unsigned long long* stamps) {
+  cudaError_t e = cudaFuncSetAttribute(knn_sweep2_kernel<NG, PNKS, STAMPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
   if (e != cudaSuccess) return e;
   const int nks = sh.kpad / 16 / sh.nsplit;
-  knn_sweep2_kernel<NG><<<grid, THREADS, sh.smem, st>>>(A, B, nks, sh.nsplit, sh.nstage, n_tiles, n_est, est_stride, qtile0, n_query,
-                                                        n_points, cs, ci);
+  knn_sweep2_kernel<NG, PNKS, STAMPS><<<grid, PNKS > 0 ? THREADS_PIPE : THREADS, sh.smem, st>>>(
+      A, B, nks, sh.nsplit, sh.nstage, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
   return cudaSuccess;
+}
+template <int NG, int PNKS>
+cudaError_t launch2(unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B, int64_t n_tiles,
+                    int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs, int32_t* ci,
+                    unsigned long long* stamps) {
+  if (stamps) return launch2s<NG, PNKS, true>(grid, sh, st, A, B, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
+  return launch2s<NG, PNKS, false>(grid, sh, st, A, B, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
+}
+template <int NG>
+cudaError_t launch2_nks(bool pipe, unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B,
+                        int64_t n_tiles, int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points,
+                        float* cs, int32_t* ci, unsigned long long* stamps) {
+  const int nks = pipe ? sh.kpad / 16 : 0;   // knn_tc2_shape only sets pipe for nsplit = 1 and these two K axes
+  if (nks == PIPE_NKS0) return launch2<NG, PIPE_NKS0>(grid, sh, st, A, B, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
+  if (nks == PIPE_NKS1) return launch2<NG, PIPE_NKS1>(grid, sh, st, A, B, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
+  return launch2<NG, 0>(grid, sh, st, A, B, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
+}
+
+// SB2_KNN_STAMPS=1: where the consumer warpgroups of one sweep spent their cycles, summed over all of them, on stderr
+int32_t report_stamps(sb2_ctx* ctx, const KnnTc2Shape& sh, bool pipe, unsigned grid, int64_t n_visit, int list_m,
+                      const unsigned long long* d_stamps) {
+  std::vector<unsigned long long> h((size_t)grid * 2 * PH_N);
+  SB2_CUDA(cudaMemcpyAsync(h.data(), d_stamps, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
+  SB2_CUDA(cudaStreamSynchronize(ctx->stream));
+  double tot[PH_N] = {0.0, 0.0, 0.0, 0.0}, all = 0.0;
+  for (size_t i = 0; i < h.size(); ++i) { tot[i % PH_N] += (double)h[i]; all += (double)h[i]; }
+  const double tiles = (double)grid * 2.0 * (double)n_visit;   // tiles examined, counted per warpgroup
+  static const char* names[PH_N] = {"wait full", "mma", "scan", "insert"};
+  fprintf(stderr, "[sb2 knn stamps] %s loop, K=%d nsplit=%d nstage=%d list=%d, %u CTAs x %lld visits: %.0f cycles/tile",
+          pipe ? "pipelined" : "single-buffer", sh.kpad, sh.nsplit, sh.nstage, list_m, grid, (long long)n_visit,
+          tiles > 0 ? all / tiles : 0.0);
+  for (int ph = 0; ph < PH_N; ++ph)
+    fprintf(stderr, ", %s %.1f%% (%.0f)", names[ph], all > 0 ? 100.0 * tot[ph] / all : 0.0, tiles > 0 ? tot[ph] / tiles : 0.0);
+  fprintf(stderr, "\n");
+  return SB2_OK;
 }
 }  // namespace
 
@@ -486,11 +645,19 @@ int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnTc2Shape& sh, const __half* Aimg, i
     SB2_CUDA(cudaGetSymbolAddress(&fp, g_knn2_front));
     SB2_CUDA(cudaMemsetAsync(fp, 0, sizeof(unsigned long long), st));
   }
+  // SB2_KNN_PIPE=0 keeps the single-buffer consumer loop where the pipelined one could run (same results, A/B timing)
+  const char* pipe_env = getenv("SB2_KNN_PIPE");
+  const bool pipe = sh.pipe && !(pipe_env && strcmp(pipe_env, "0") == 0);
+  const char* stamps_env = getenv("SB2_KNN_STAMPS");
+  ScratchScope scr(ctx);
+  unsigned long long* stamps = nullptr;
+  if (stamps_env && strcmp(stamps_env, "1") == 0) SB2_TRY(scr.alloc(&stamps, (size_t)grid * 2 * PH_N));
   cudaError_t le;
-  if (list_m == 64) le = launch2<2>(grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, a_tile0, n_query, np, cand_score, cand_idx);
-  else le = launch2<4>(grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, a_tile0, n_query, np, cand_score, cand_idx);
+  if (list_m == 64) le = launch2_nks<2>(pipe, grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, a_tile0, n_query, np, cand_score, cand_idx, stamps);
+  else le = launch2_nks<4>(pipe, grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, a_tile0, n_query, np, cand_score, cand_idx, stamps);
   SB2_CUDA(le);
   SB2_LAUNCH_CHECK(ctx);
+  if (stamps) SB2_TRY(report_stamps(ctx, sh, pipe, grid, n_tiles + n_est, list_m, stamps));
   return SB2_OK;
 }
 

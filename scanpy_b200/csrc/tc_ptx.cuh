@@ -49,6 +49,20 @@ __device__ __forceinline__ uint64_t wgmma_desc(uint32_t saddr, uint32_t lbo, uin
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// per-warpgroup register budget (executed by all warps of a warpgroup); inc blocks until dec elsewhere freed enough
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+// wait until at most N committed groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// pins every access to an accumulator on its side of a wgmma fence / wait: the compiler may not move reads of d
+// above the wait that completes the group writing d, nor writes below the issue of a group reading it
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[64]) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
 // D[64x128] (+)= A[64x16] B[128x16]^T, fp16 operands from shared memory (both K-major), fp32 accumulators in registers.
 // scale_d = 0 overwrites D.  Fragment of thread t of the warpgroup (warp w = t / 32, lane l): d[4i + 2h + e] is row
