@@ -27,7 +27,7 @@
 //                 setmaxnreg can hand their registers to the consumers)
 //   Starting threshold: the first n/16 visits sweep every 16th tile and keep the 6 largest chunk maxima per (row,
 //   sub-list); the four sub-lists of a row (four lanes of one warp) are merged by shuffles once and the 6th largest of
-//   the 24 seeds all four (rank ~96 of the row).
+//   the 24 seeds all four (rank ~96 of the row; SB2_KNN_EST_RANK picks another of the six).
 //   Sweep front: CTAs walk the candidate tiles cyclically, starting where the running CTAs currently are (g_knn2_front).
 #include <cuda_fp16.h>
 #include <float.h>
@@ -56,7 +56,8 @@ constexpr int PROD_REGS = 40, CONS_REGS = 232;
 constexpr int PIPE_NKS0 = 4, PIPE_NKS1 = 10;
 static_assert(128 * PROD_REGS + 256 * CONS_REGS <= 65536 / THREADS_PIPE / 8 * 8 * THREADS_PIPE, "register file");
 constexpr int NSUB = 4;            // sub-lists per query row
-constexpr int EST_R = 6;
+constexpr int EST_R = 6;           // chunk maxima an estimate keeps per (row, sub-list)
+constexpr int EST_STRIDE = 16;     // the estimate samples every 16th candidate tile
 constexpr uint32_t SBO = 128;              // bytes between 8-row groups (core matrices contiguous)
 constexpr uint32_t LBO = QM * 16;          // bytes between K-chunks of a 128-row image  [kc][row-group][8][8]
 static_assert(QM == CN, "query and candidate images share one layout");
@@ -191,46 +192,48 @@ __device__ __forceinline__ float max8u(const uint32_t* v) {
                fmax3(__uint_as_float(v[3]), __uint_as_float(v[4]), __uint_as_float(v[5])),
                fmaxf(__uint_as_float(v[6]), __uint_as_float(v[7])));
 }
-// examine one 32-value chunk of the row (values already in registers; value m is candidate cand0 + 8 (m / 2) + m % 2,
-// the columns one thread holds in the wgmma accumulator fragment).  Fast path: a max tree (four independent quarter
-// maxima, so the latencies overlap) and one compare.  Rare path: visit the quarters whose
-// maximum beats tau, copy the quarter's eight values aside and pull its maxima out one by one.  The quarter loop is
-// NOT unrolled: one copy of the extraction and insertion code per call site keeps the kernel in the instruction caches.
+// A thread examines one 32-value chunk of each of its two rows per tile (values already in registers; value m is
+// candidate cand0 + 8 (m / 2) + m % 2, the columns one thread holds in the wgmma accumulator fragment).
+// Fast path (chunk_max): a max tree of four independent quarter maxima (their latencies overlap) and one compare per row.
+// Rare path (insert_hits), entered by the whole warp when any of its 64 (row, sub-list) pairs has a hit: a 32-bit mask
+// of the values above tau (one compare each), walked lowest bit first with __ffs; each set bit's value is picked out of
+// the registers by a five-level select tree and inserted if it still beats tau (every insertion raises tau).  So the
+// values of a chunk go in column by column, not largest first: the scores a sub-list ends with do not depend on that
+// order, only which of several EQUAL scores at tau it keeps, and those lie below every score the certificate accepts
+// (a row whose k-th score ties tau is re-swept or scanned exactly), so the final (idx, dist) do not either.
 // stamp(PH_SCAN) / stamp(PH_INSERT) bracket the rare path for the opt-in phase stamps (no-ops when they are off).
 enum { PH_WAIT = 0, PH_MMA, PH_SCAN, PH_INSERT, PH_N };
-template <int NG, class Stamp>
-__device__ __forceinline__ void scan_chunk(SubList<NG>& L, int32_t* __restrict__ id, const uint32_t (&v)[32], int32_t cand0,
-                                           int32_t n_points, const Stamp& stamp) {
-  const float h0 = max8u(&v[0]), h1 = max8u(&v[8]), h2 = max8u(&v[16]), h3 = max8u(&v[24]);
-  stamp(PH_SCAN);
-  if (fmaxf(fmax3(h0, h1, h2), h3) > L.tau) {
-#pragma unroll 1
-    for (int q = 0; q < 4; ++q) {
-      float hq = q == 0 ? h0 : (q == 1 ? h1 : (q == 2 ? h2 : h3));
-      if (hq > L.tau) {
-        uint32_t w[8];
+// per (CTA, warpgroup) the stamps buffer holds the PH_N phase totals and two counters of the STAMPS instantiation:
+// warp-tiles of the sweep proper on which a warp took the rare path, and insertions into the warpgroup's sub-lists
+enum { CNT_RARE = PH_N, CNT_INSERT, ST_N };
+__device__ __forceinline__ float chunk_max(const uint32_t (&v)[32]) {
+  return fmaxf(fmax3(max8u(&v[0]), max8u(&v[8]), max8u(&v[16])), max8u(&v[24]));
+}
+template <int NG, bool COUNT>
+__device__ __forceinline__ void insert_hits(SubList<NG>& L, int32_t* __restrict__ id, const uint32_t (&v)[32], int32_t cand0,
+                                            int32_t n_points, unsigned& n_ins) {
+  uint32_t m = 0;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) w[i] = q == 0 ? v[i] : (q == 1 ? v[8 + i] : (q == 2 ? v[16 + i] : v[24 + i]));
-        do {
-          int j = 0;
-          bool found = false;
-          const uint32_t mb = __float_as_uint(hq);
+  for (int i = 0; i < 32; ++i) m |= (__uint_as_float(v[i]) > L.tau ? 1u : 0u) << i;
+  while (m) {
+    const int j = __ffs(m) - 1;
+    m &= m - 1;
+    uint32_t s[16];   // v[j]: registers cannot be indexed at run time
 #pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            const bool hset = !found && (w[jj] == mb);
-            j = hset ? jj : j;
-            w[jj] = hset ? 0xff800000u : w[jj];  // knock the maximum out (-inf)
-            found |= hset;
-          }
-          const int m = q * 8 + j;                          // value m of the chunk is column 8 (m / 2) + m % 2
-          const int32_t cand = cand0 + ((m >> 1) << 3) + (m & 1);
-          if (cand < n_points) list_insert(L, id, hq, cand);
-          hq = max8u(w);
-        } while (hq > L.tau);
-      }
+    for (int i = 0; i < 16; ++i) s[i] = (j & 1) ? v[2 * i + 1] : v[2 * i];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s[i] = (j & 2) ? s[2 * i + 1] : s[2 * i];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) s[i] = (j & 4) ? s[2 * i + 1] : s[2 * i];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) s[i] = (j & 8) ? s[2 * i + 1] : s[2 * i];
+    const float x = __uint_as_float((j & 16) ? s[1] : s[0]);
+    const int32_t cand = cand0 + ((j >> 1) << 3) + (j & 1);
+    if (x > L.tau && cand < n_points) {
+      list_insert(L, id, x, cand);
+      if (COUNT) ++n_ins;
     }
   }
-  stamp(PH_INSERT);
 }
 // estimate phase: keep the EST_R largest values seen (sorted descending), branch-free
 template <int LEN>
@@ -244,7 +247,7 @@ __device__ __forceinline__ void est_push(float (&est)[LEN], float cm) {
 }
 template <int LEN>
 __device__ __forceinline__ void est_chunk(float (&est)[LEN], const uint32_t (&v)[32]) {
-  est_push(est, fmaxf(fmax3(max8u(&v[0]), max8u(&v[8]), max8u(&v[16])), max8u(&v[24])));
+  est_push(est, chunk_max(v));
 }
 
 // nks = k-steps (16 columns of the K axis) per staged slice, nsplit = slices per candidate image.
@@ -263,15 +266,17 @@ __device__ unsigned long long g_knn2_front;   // sweep-proper visits of all CTAs
 //   registers rebalanced).  The k-step count is a template argument because ptxas serialises every wgmma of the kernel
 //   when a loop with a run-time trip count issues them while another group is in flight.
 // STAMPS: lane 0 of warp 0 of each consumer warpgroup adds up clock64() per phase (PH_WAIT on full[s], PH_MMA issue to
-//   end of the wgmma wait, PH_SCAN examination incl. estimate / seeding / release, PH_INSERT the rare path of
-//   scan_chunk) in shared memory and writes stamps[(cta * 2 + warpgroup) * PH_N + phase] at the end.  A template
+//   end of the wgmma wait, PH_SCAN examination incl. estimate / seeding / release, PH_INSERT the rare path,
+//   insert_hits) in shared memory and writes stamps[(cta * 2 + warpgroup) * ST_N + phase] at the end; every warp adds
+//   its rare-path tiles and insertions to the CNT_RARE / CNT_INSERT slots.  A template
 //   argument, not a run-time test: even never-taken uniform branches inside the scan cost the single-buffer loop 8 %
 //   (they split the examination into blocks the scheduler cannot interleave).
 template <int NG, int PNKS, bool STAMPS>
 __global__ void __launch_bounds__(PNKS > 0 ? THREADS_PIPE : THREADS, 1)
 knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bimg, int nks, int nsplit, int nstage,
-                  int64_t n_btiles, int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points,
-                  float* __restrict__ cand_score, int32_t* __restrict__ cand_idx, unsigned long long* __restrict__ stamps) {
+                  int64_t n_btiles, int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query,
+                  int32_t n_points, float* __restrict__ cand_score, int32_t* __restrict__ cand_idx,
+                  unsigned long long* __restrict__ stamps) {
   constexpr bool PIPE = PNKS > 0;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   const uint32_t part_b = (uint32_t)(CN * 16 * 2) * (uint32_t)nks;     // bytes per staged K-slice of a candidate image
@@ -376,6 +381,8 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
     }
   };
 
+  unsigned n_ins = 0, n_rare = 0;   // STAMPS: this thread's insertions, this warp's rare-path tiles
+
   // everything a warpgroup does with the scores of visit c once they are in acc
   const auto examine = [&](const float (&acc)[64], int c) {
     if (c == n_est_i) {
@@ -395,8 +402,14 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
           }
         }
       }
-      const float t0 = valid0 ? L0.ls[EST_R - 1] : INFINITY;  // rows past n_query never accept anything
-      const float t1 = valid1 ? L1.ls[EST_R - 1] : INFINITY;
+      float e0 = L0.ls[0], e1 = L1.ls[0];    // the est_rank-th largest of the merged chunk maxima
+#pragma unroll
+      for (int i = 1; i < EST_R; ++i) {
+        e0 = i < est_rank ? L0.ls[i] : e0;
+        e1 = i < est_rank ? L1.ls[i] : e1;
+      }
+      const float t0 = valid0 ? e0 : INFINITY;  // rows past n_query never accept anything
+      const float t1 = valid1 ? e1 : INFINITY;
 #pragma unroll
       for (int i = 0; i < LS; ++i) { L0.ls[i] = t0; L1.ls[i] = t1; }
 #pragma unroll
@@ -416,8 +429,14 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
       est_chunk(L0.ls, v0);
       est_chunk(L1.ls, v1);
     } else {
-      scan_chunk(L0, id0, v0, cbase, n_points, stamp);
-      scan_chunk(L1, id1, v1, cbase, n_points, stamp);
+      const bool hit0 = chunk_max(v0) > L0.tau, hit1 = chunk_max(v1) > L1.tau;
+      stamp(PH_SCAN);
+      if (__builtin_expect(__any_sync(0xffffffffu, hit0 || hit1), 0)) {
+        if (STAMPS) ++n_rare;
+        if (hit0) insert_hits<NG, STAMPS>(L0, id0, v0, cbase, n_points, n_ins);
+        if (hit1) insert_hits<NG, STAMPS>(L1, id1, v1, cbase, n_points, n_ins);
+      }
+      stamp(PH_INSERT);
       if ((c & 15) == 0 && warp == 0 && lane == 0) atomicAdd(&g_knn2_front, 1ull);   // 16 more visits of the pack
       cbase += CN;
       if (++ctile == n_bt) { ctile = 0; cbase = 2 * sl; }
@@ -512,8 +531,16 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
       stamp(PH_SCAN);
     }
   }
-  if (stamp_on && lane == 0) {
-    for (int ph = 0; ph < PH_N; ++ph) stamps[((size_t)blockIdx.x * 2 + g) * PH_N + ph] = my_st[ph];
+  if (STAMPS) {
+    unsigned long long* st = stamps + ((size_t)blockIdx.x * 2 + g) * ST_N;   // zeroed by the host
+    const unsigned ins = __reduce_add_sync(0xffffffffu, n_ins);
+    if (lane == 0) {
+      atomicAdd(&st[CNT_RARE], (unsigned long long)n_rare);
+      atomicAdd(&st[CNT_INSERT], (unsigned long long)ins);
+    }
+    if (stamp_on && lane == 0) {
+      for (int ph = 0; ph < PH_N; ++ph) st[ph] = my_st[ph];
+    }
   }
   if (valid0) {
 #pragma unroll
@@ -578,40 +605,47 @@ int32_t knn_tc2_build_images(sb2_ctx* ctx, const KnnTc2Shape& sh, const float* d
 namespace {
 template <int NG, int PNKS, bool STAMPS>
 cudaError_t launch2s(unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B, int64_t n_tiles,
-                     int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs, int32_t* ci,
-                     unsigned long long* stamps) {
+                     int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs,
+                     int32_t* ci, unsigned long long* stamps) {
   cudaError_t e = cudaFuncSetAttribute(knn_sweep2_kernel<NG, PNKS, STAMPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
   if (e != cudaSuccess) return e;
   const int nks = sh.kpad / 16 / sh.nsplit;
   knn_sweep2_kernel<NG, PNKS, STAMPS><<<grid, PNKS > 0 ? THREADS_PIPE : THREADS, sh.smem, st>>>(
-      A, B, nks, sh.nsplit, sh.nstage, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
+      A, B, nks, sh.nsplit, sh.nstage, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
   return cudaSuccess;
 }
 template <int NG, int PNKS>
 cudaError_t launch2(unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B, int64_t n_tiles,
-                    int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs, int32_t* ci,
-                    unsigned long long* stamps) {
-  if (stamps) return launch2s<NG, PNKS, true>(grid, sh, st, A, B, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
-  return launch2s<NG, PNKS, false>(grid, sh, st, A, B, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
+                    int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs,
+                    int32_t* ci, unsigned long long* stamps) {
+  if (stamps)
+    return launch2s<NG, PNKS, true>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
+  return launch2s<NG, PNKS, false>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
 }
 template <int NG>
 cudaError_t launch2_nks(bool pipe, unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B,
-                        int64_t n_tiles, int64_t n_est, int64_t est_stride, int64_t qtile0, int64_t n_query, int32_t n_points,
-                        float* cs, int32_t* ci, unsigned long long* stamps) {
+                        int64_t n_tiles, int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query,
+                        int32_t n_points, float* cs, int32_t* ci, unsigned long long* stamps) {
   const int nks = pipe ? sh.kpad / 16 : 0;   // knn_tc2_shape only sets pipe for nsplit = 1 and these two K axes
-  if (nks == PIPE_NKS0) return launch2<NG, PIPE_NKS0>(grid, sh, st, A, B, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
-  if (nks == PIPE_NKS1) return launch2<NG, PIPE_NKS1>(grid, sh, st, A, B, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
-  return launch2<NG, 0>(grid, sh, st, A, B, n_tiles, n_est, est_stride, qtile0, n_query, n_points, cs, ci, stamps);
+  if (nks == PIPE_NKS0)
+    return launch2<NG, PIPE_NKS0>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
+  if (nks == PIPE_NKS1)
+    return launch2<NG, PIPE_NKS1>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
+  return launch2<NG, 0>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
 }
 
-// SB2_KNN_STAMPS=1: where the consumer warpgroups of one sweep spent their cycles, summed over all of them, on stderr
-int32_t report_stamps(sb2_ctx* ctx, const KnnTc2Shape& sh, bool pipe, unsigned grid, int64_t n_visit, int list_m,
-                      const unsigned long long* d_stamps) {
-  std::vector<unsigned long long> h((size_t)grid * 2 * PH_N);
+// SB2_KNN_STAMPS=1: where the consumer warpgroups of one sweep spent their cycles, summed over all of them, and how
+// often they left the fast path, on stderr
+int32_t report_stamps(sb2_ctx* ctx, const KnnTc2Shape& sh, bool pipe, unsigned grid, int64_t n_visit, int64_t n_est, int64_t n_query,
+                      int list_m, const unsigned long long* d_stamps) {
+  std::vector<unsigned long long> h((size_t)grid * 2 * ST_N);
   SB2_CUDA(cudaMemcpyAsync(h.data(), d_stamps, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
   SB2_CUDA(cudaStreamSynchronize(ctx->stream));
-  double tot[PH_N] = {0.0, 0.0, 0.0, 0.0}, all = 0.0;
-  for (size_t i = 0; i < h.size(); ++i) { tot[i % PH_N] += (double)h[i]; all += (double)h[i]; }
+  double tot[ST_N] = {}, all = 0.0;
+  for (size_t i = 0; i < h.size(); ++i) {
+    tot[i % ST_N] += (double)h[i];
+    if (i % ST_N < PH_N) all += (double)h[i];
+  }
   const double tiles = (double)grid * 2.0 * (double)n_visit;   // tiles examined, counted per warpgroup
   static const char* names[PH_N] = {"wait full", "mma", "scan", "insert"};
   fprintf(stderr, "[sb2 knn stamps] %s loop, K=%d nsplit=%d nstage=%d list=%d, %u CTAs x %lld visits: %.0f cycles/tile",
@@ -619,7 +653,11 @@ int32_t report_stamps(sb2_ctx* ctx, const KnnTc2Shape& sh, bool pipe, unsigned g
           tiles > 0 ? all / tiles : 0.0);
   for (int ph = 0; ph < PH_N; ++ph)
     fprintf(stderr, ", %s %.1f%% (%.0f)", names[ph], all > 0 ? 100.0 * tot[ph] / all : 0.0, tiles > 0 ? tot[ph] / tiles : 0.0);
-  fprintf(stderr, "\n");
+  // the rare path: share of the sweep proper's warp-tiles (8 consumer warps per CTA) on which a warp took it, and the
+  // insertions per query row (four sub-lists)
+  const double warp_tiles = (double)grid * NCONS * (double)(n_visit - n_est);
+  fprintf(stderr, ", rare-path tiles %.2f%%, insertions/row %.1f\n", warp_tiles > 0 ? 100.0 * tot[CNT_RARE] / warp_tiles : 0.0,
+          n_query > 0 ? tot[CNT_INSERT] / (double)n_query : 0.0);
   return SB2_OK;
 }
 }  // namespace
@@ -631,12 +669,17 @@ int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnTc2Shape& sh, const __half* Aimg, i
   const int64_t n_tiles = ceil_div64(n_points, CN);
   const int64_t q_ctas = ceil_div64(n_query, QM);
   SB2_CHECK_ARG(list_m == 64 || list_m == 128, "list_m must be 64 or 128 (four sub-lists of 16 or 32)");
-  // threshold estimate: the 6th largest of the row's chunk maxima over every est_stride-th tile sits at about rank
-  // EST_R * est_stride of the row; aim at ~96 (1.5 x the 64 proposals kept), i.e. a 1/16 sample
-  int64_t est_stride = 96 / EST_R, n_est = n_tiles / est_stride;
+  // threshold estimate: the est_rank-th largest of the row's chunk maxima over every est_stride-th tile sits at about
+  // rank est_rank * est_stride of the row
+  int64_t est_stride = EST_STRIDE, n_est = n_tiles / est_stride;
   const char* est_env = getenv("SB2_KNN_EST");
   if (est_env) est_stride = atoi(est_env) > 0 ? atoi(est_env) : est_stride, n_est = atoi(est_env) > 0 ? n_tiles / est_stride : 0;
   if (n_tiles < 32 * est_stride || !estimate || !sh.est) n_est = 0;  // small problems / re-sweeps: cold start
+  // the sub-lists start at the est_rank-th largest of the row's sampled chunk maxima, rank ~96 of the row by default:
+  // on the 1.3M x 50 benchmark (k = 15) every rank below 6 sends more rows to the split-precision re-sweep (rank 5:
+  // 7x as many, rank 4: 46x) than it saves in insertions.  SB2_KNN_EST_RANK=1..6 picks another (tests, A/B timing).
+  int est_rank = EST_R;
+  if (const char* r_env = getenv("SB2_KNN_EST_RANK")) est_rank = atoi(r_env) >= 1 && atoi(r_env) <= EST_R ? atoi(r_env) : est_rank;
   if (issued_flops) *issued_flops += 2.0 * (double)(q_ctas * QM) * (double)((n_tiles + n_est) * CN) * (double)sh.kpad;
   const unsigned grid = (unsigned)q_ctas;
   const int32_t np = (int32_t)n_points;
@@ -651,13 +694,18 @@ int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnTc2Shape& sh, const __half* Aimg, i
   const char* stamps_env = getenv("SB2_KNN_STAMPS");
   ScratchScope scr(ctx);
   unsigned long long* stamps = nullptr;
-  if (stamps_env && strcmp(stamps_env, "1") == 0) SB2_TRY(scr.alloc(&stamps, (size_t)grid * 2 * PH_N));
+  if (stamps_env && strcmp(stamps_env, "1") == 0) {
+    SB2_TRY(scr.alloc(&stamps, (size_t)grid * 2 * ST_N));
+    SB2_CUDA(cudaMemsetAsync(stamps, 0, (size_t)grid * 2 * ST_N * sizeof(unsigned long long), st));
+  }
   cudaError_t le;
-  if (list_m == 64) le = launch2_nks<2>(pipe, grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, a_tile0, n_query, np, cand_score, cand_idx, stamps);
-  else le = launch2_nks<4>(pipe, grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, a_tile0, n_query, np, cand_score, cand_idx, stamps);
+  if (list_m == 64)
+    le = launch2_nks<2>(pipe, grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, est_rank, a_tile0, n_query, np, cand_score, cand_idx, stamps);
+  else
+    le = launch2_nks<4>(pipe, grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, est_rank, a_tile0, n_query, np, cand_score, cand_idx, stamps);
   SB2_CUDA(le);
   SB2_LAUNCH_CHECK(ctx);
-  if (stamps) SB2_TRY(report_stamps(ctx, sh, pipe, grid, n_tiles + n_est, list_m, stamps));
+  if (stamps) SB2_TRY(report_stamps(ctx, sh, pipe, grid, n_tiles + n_est, n_est, n_query, list_m, stamps));
   return SB2_OK;
 }
 
