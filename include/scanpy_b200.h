@@ -303,6 +303,32 @@ int32_t sb2_pearson_residuals(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_
                               const double* d_gene, const double* d_cell, double total, double clip, double theta,
                               int32_t out_f64, void* d_out);
 
+/* ---- sc.pp.combat (src/scanpy/preprocessing/_combat.py:71-289; csrc/combat.cu) ----
+ * X is a block of `rows` rows as for regress_out: dense (d_x) or CSR arrays (d_indptr pointing at the block's first row,
+ * entry offsets absolute; sorted column indices, no duplicates), float32 (is_f64 = 0) or float64 values.  DᵀX is
+ * sb2_regress_col_sums (grouped for the batch columns, weighted for the covariate columns).  With stand_mean[i,j] =
+ * d_grand[j] + sum_k cov[i,k] d_beta[k*g+j] (cov fp64 [rows x p], p <= 32; p = 0: d_cov, d_beta may be NULL) and
+ * r = x - stand_mean, all in fp64:
+ * sb2_combat_moments <- the per-batch statistics of _standardize_data / combat for one batch.  Row k of the call is X row
+ *                       d_order[k] (d_order NULL: row k of the block; with CSR, d_indptr then indexes d_order's rows),
+ *                       d_cov row k its covariates.  Merges into d_acc fp64 [3 x g] (zeroed before the first call of a
+ *                       batch): row 0 the count, 1 the mean of r, 2 the sum of squared deviations of r.  Blocks of one
+ *                       batch must be consecutive, and all but the last a multiple of SB2_COMBAT_TILE_ROWS rows: the
+ *                       result then has the same bits as one call over the batch.
+ * sb2_combat_adjust  <- the parametric adjustment: d_out[i*g+j] (float64) = ((s - gamma[b*g+j]) / dsq[b*g+j]) *
+ *                       sqrt_vp[j] + stand_mean[i,j] with b = d_batch[i], s = r / sqrt_vp[j] (0 where sqrt_vp[j] == 0);
+ *                       d_cov row i belongs to block row i. */
+#define SB2_COMBAT_TILE_ROWS 1024
+int32_t sb2_combat_moments(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f64, const void* d_x,
+                           const int64_t* d_indptr, const int32_t* d_indices, const void* d_data,
+                           const int64_t* d_order, const double* d_cov, int32_t p, const double* d_grand,
+                           const double* d_beta, double* d_acc);
+int32_t sb2_combat_adjust(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f64, const void* d_x,
+                          const int64_t* d_indptr, const int32_t* d_indices, const void* d_data,
+                          const int32_t* d_batch, const double* d_cov, int32_t p, const double* d_grand,
+                          const double* d_beta, const double* d_sqrt_vp, const double* d_gamma, const double* d_dsq,
+                          double* d_out);
+
 
 /* ---- extreme eigenpairs of diag(s) A diag(s), A symmetric fp32 CSR (csrc/eigs.cu: thick-restart Lanczos, fp64) ----
  * Replaces `scipy.sparse.linalg.eigsh(matrix.astype(float64), k=n_comps, which='LM', v0=...)` in

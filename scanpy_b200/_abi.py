@@ -133,6 +133,11 @@ SIGNATURES = {
                                            c_void_p, c_void_p, c_void_p, c_double, c_double, c_double, c_void_p]),
     "sb2_pearson_residuals": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
                                         c_void_p, c_void_p, c_double, c_double, c_double, c_int32, c_void_p]),
+    "sb2_combat_moments": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
+    "sb2_combat_adjust": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p]),
 }
 
 _lib = None

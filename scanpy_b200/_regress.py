@@ -53,7 +53,13 @@ _DeviceX = _ops.DeviceX
 
 def _col_sums(dx: _DeviceX, n: int, g: int, *, w=None, group=None, n_groups: int = 0):
     """Weighted (`w`, n x p fp64): WᵀX [p x g]; grouped (`group`, int32 [n] in [0, n_groups)): the per-group column sums
-    [n_groups x g].  Also the per-gene min, max and NaN flag."""
+    [n_groups x g].  Also the flag of the genes whose values are all equal (no NaN)."""
+    acc, cmin, cmax, cnan = _col_sums_stats(dx, n, g, w=w, group=group, n_groups=n_groups)
+    return acc, (cnan == 0) & (cmin == cmax)
+
+
+def _col_sums_stats(dx: _DeviceX, n: int, g: int, *, w=None, group=None, n_groups: int = 0):
+    """As `_col_sums`, with the per-gene min, max and NaN flag (int32) themselves."""
     import torch
 
     ctx = _abi.default_context()
@@ -82,8 +88,7 @@ def _col_sums(dx: _DeviceX, n: int, g: int, *, w=None, group=None, n_groups: int
                                            width if w is not None else 0, ptr(d_group), ptr(d_order), n_groups,
                                            ptr(acc), ptr(cmin), ptr(cmax), ptr(cnan)))
     acc, cmin, cmax, cnan = _ops._to_host(acc, cmin, cmax, cnan)
-    constant = (cnan == 0) & (cmin == cmax)
-    return acc.reshape(width, g), constant
+    return acc.reshape(width, g), cmin, cmax, cnan
 
 
 def _residual(dx: _DeviceX, n: int, g: int, out_dtype: np.dtype, *, w=None, coef=None, codes=None, means=None, b0=None,

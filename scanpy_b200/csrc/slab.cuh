@@ -1,4 +1,4 @@
-// slab.cuh — the column-slab scheme of the dense per-gene passes (regress.cu, pearson.cu).
+// slab.cuh — the column-slab scheme of the dense per-gene passes (regress.cu, pearson.cu, combat.cu).
 //
 // One CTA owns a SLAB_THREADS-column slab of a block of rows and each thread one column.  A CSR input is read in place:
 // the CTA binary-searches its slab in each of SLAB_ROWS rows (column indices sorted, no duplicates) and scatters the
