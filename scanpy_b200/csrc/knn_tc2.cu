@@ -194,7 +194,17 @@ __device__ __forceinline__ float max8u(const uint32_t* v) {
 }
 // A thread examines one 32-value chunk of each of its two rows per tile (values already in registers; value m is
 // candidate cand0 + 8 (m / 2) + m % 2, the columns one thread holds in the wgmma accumulator fragment).
-// Fast path (chunk_max): a max tree of four independent quarter maxima (their latencies overlap) and one compare per row.
+// Fast path: "does anything in the chunk beat tau", one max tree and one compare per row.
+//   chunk_imax (ISCAN, the default): the signed-integer maximum of the 32 raw bit patterns, a ternary tree of Hopper's
+//     three-input integer max (VIMNMX3: 15 of them and one VIMNMX, against 31 FMNMX), compared with tau's bit pattern.
+//     Exact whenever tau's sign bit is clear: a float above a non-negative tau is positive, positive floats order like
+//     their patterns, and a negative value's pattern is a negative integer, below every non-negative pattern, so where
+//     the negative values fall among themselves never matters.  Scores are finite (padding candidates score -60000),
+//     and tau = +inf (rows past n_query) is above every finite pattern.
+//   chunk_max: the float maximum, a tree of four independent quarter maxima.  The estimate phase needs the value itself,
+//     and the hit test needs it while tau's sign bit is set (a cold start begins at -inf; rows near the origin keep a
+//     negative tau): a warp with such a row takes the rare branch and redoes the test of both rows in floats there, so
+//     the fast path pays one OR and one compare for the rule.
 // Rare path (insert_hits), entered by the whole warp when any of its 64 (row, sub-list) pairs has a hit: a 32-bit mask
 // of the values above tau (one compare each), walked lowest bit first with __ffs; each set bit's value is picked out of
 // the registers by a five-level select tree and inserted if it still beats tau (every insertion raises tau).  So the
@@ -208,6 +218,14 @@ enum { PH_WAIT = 0, PH_MMA, PH_SCAN, PH_INSERT, PH_N };
 enum { CNT_RARE = PH_N, CNT_INSERT, ST_N };
 __device__ __forceinline__ float chunk_max(const uint32_t (&v)[32]) {
   return fmaxf(fmax3(max8u(&v[0]), max8u(&v[8]), max8u(&v[16])), max8u(&v[24]));
+}
+__device__ __forceinline__ int chunk_imax(const uint32_t (&v)[32]) {
+  int a[10];
+#pragma unroll
+  for (int i = 0; i < 10; ++i) a[i] = __vimax3_s32((int)v[3 * i], (int)v[3 * i + 1], (int)v[3 * i + 2]);
+  const int b0 = __vimax3_s32(a[0], a[1], a[2]), b1 = __vimax3_s32(a[3], a[4], a[5]), b2 = __vimax3_s32(a[6], a[7], a[8]);
+  const int b3 = __vimax3_s32(a[9], (int)v[30], (int)v[31]);
+  return max(__vimax3_s32(b0, b1, b2), b3);
 }
 template <int NG, bool COUNT>
 __device__ __forceinline__ void insert_hits(SubList<NG>& L, int32_t* __restrict__ id, const uint32_t (&v)[32], int32_t cand0,
@@ -271,7 +289,8 @@ __device__ unsigned long long g_knn2_front;   // sweep-proper visits of all CTAs
 //   its rare-path tiles and insertions to the CNT_RARE / CNT_INSERT slots.  A template
 //   argument, not a run-time test: even never-taken uniform branches inside the scan cost the single-buffer loop 8 %
 //   (they split the examination into blocks the scheduler cannot interleave).
-template <int NG, int PNKS, bool STAMPS>
+// ISCAN: the fast path's hit test on the bit patterns (chunk_imax); false keeps the float max tree (SB2_KNN_SCAN=float).
+template <int NG, int PNKS, bool STAMPS, bool ISCAN>
 __global__ void __launch_bounds__(PNKS > 0 ? THREADS_PIPE : THREADS, 1)
 knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bimg, int nks, int nsplit, int nstage,
                   int64_t n_btiles, int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query,
@@ -429,12 +448,31 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
       est_chunk(L0.ls, v0);
       est_chunk(L1.ls, v1);
     } else {
-      const bool hit0 = chunk_max(v0) > L0.tau, hit1 = chunk_max(v1) > L1.tau;
+      bool hit0, hit1, redo = false;
+      if constexpr (ISCAN) {
+        const int t0 = __float_as_int(L0.tau), t1 = __float_as_int(L1.tau);
+        hit0 = chunk_imax(v0) > t0;
+        hit1 = chunk_imax(v1) > t1;
+        redo = (t0 | t1) < 0;   // a sign bit is set: the integer test of this thread's rows proves nothing
+      } else {
+        hit0 = chunk_max(v0) > L0.tau;
+        hit1 = chunk_max(v1) > L1.tau;
+      }
       stamp(PH_SCAN);
-      if (__builtin_expect(__any_sync(0xffffffffu, hit0 || hit1), 0)) {
-        if (STAMPS) ++n_rare;
-        if (hit0) insert_hits<NG, STAMPS>(L0, id0, v0, cbase, n_points, n_ins);
-        if (hit1) insert_hits<NG, STAMPS>(L1, id1, v1, cbase, n_points, n_ins);
+      if (__builtin_expect(__any_sync(0xffffffffu, hit0 || hit1 || redo), 0)) {
+        bool rare = true;
+        if constexpr (ISCAN) {
+          if (__any_sync(0xffffffffu, redo)) {
+            hit0 = chunk_max(v0) > L0.tau;
+            hit1 = chunk_max(v1) > L1.tau;
+            rare = __any_sync(0xffffffffu, hit0 || hit1);
+          }
+        }
+        if (rare) {
+          if (STAMPS) ++n_rare;
+          if (hit0) insert_hits<NG, STAMPS>(L0, id0, v0, cbase, n_points, n_ins);
+          if (hit1) insert_hits<NG, STAMPS>(L1, id1, v1, cbase, n_points, n_ins);
+        }
       }
       stamp(PH_INSERT);
       if ((c & 15) == 0 && warp == 0 && lane == 0) atomicAdd(&g_knn2_front, 1ull);   // 16 more visits of the pack
@@ -603,35 +641,35 @@ int32_t knn_tc2_build_images(sb2_ctx* ctx, const KnnTc2Shape& sh, const float* d
 }
 
 namespace {
-template <int NG, int PNKS, bool STAMPS>
+template <int NG, int PNKS, bool STAMPS, bool ISCAN>
 cudaError_t launch2s(unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B, int64_t n_tiles,
                      int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs,
                      int32_t* ci, unsigned long long* stamps) {
-  cudaError_t e = cudaFuncSetAttribute(knn_sweep2_kernel<NG, PNKS, STAMPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
+  cudaError_t e = cudaFuncSetAttribute(knn_sweep2_kernel<NG, PNKS, STAMPS, ISCAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
   if (e != cudaSuccess) return e;
   const int nks = sh.kpad / 16 / sh.nsplit;
-  knn_sweep2_kernel<NG, PNKS, STAMPS><<<grid, PNKS > 0 ? THREADS_PIPE : THREADS, sh.smem, st>>>(
+  knn_sweep2_kernel<NG, PNKS, STAMPS, ISCAN><<<grid, PNKS > 0 ? THREADS_PIPE : THREADS, sh.smem, st>>>(
       A, B, nks, sh.nsplit, sh.nstage, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
   return cudaSuccess;
 }
-template <int NG, int PNKS>
+template <int NG, int PNKS, bool ISCAN>
 cudaError_t launch2(unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B, int64_t n_tiles,
                     int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs,
                     int32_t* ci, unsigned long long* stamps) {
   if (stamps)
-    return launch2s<NG, PNKS, true>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
-  return launch2s<NG, PNKS, false>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
+    return launch2s<NG, PNKS, true, ISCAN>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
+  return launch2s<NG, PNKS, false, ISCAN>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
 }
-template <int NG>
+template <int NG, bool ISCAN>
 cudaError_t launch2_nks(bool pipe, unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B,
                         int64_t n_tiles, int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query,
                         int32_t n_points, float* cs, int32_t* ci, unsigned long long* stamps) {
   const int nks = pipe ? sh.kpad / 16 : 0;   // knn_tc2_shape only sets pipe for nsplit = 1 and these two K axes
   if (nks == PIPE_NKS0)
-    return launch2<NG, PIPE_NKS0>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
+    return launch2<NG, PIPE_NKS0, ISCAN>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
   if (nks == PIPE_NKS1)
-    return launch2<NG, PIPE_NKS1>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
-  return launch2<NG, 0>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
+    return launch2<NG, PIPE_NKS1, ISCAN>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
+  return launch2<NG, 0, ISCAN>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
 }
 
 // SB2_KNN_STAMPS=1: where the consumer warpgroups of one sweep spent their cycles, summed over all of them, and how
@@ -698,11 +736,13 @@ int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnTc2Shape& sh, const __half* Aimg, i
     SB2_TRY(scr.alloc(&stamps, (size_t)grid * 2 * ST_N));
     SB2_CUDA(cudaMemsetAsync(stamps, 0, (size_t)grid * 2 * ST_N * sizeof(unsigned long long), st));
   }
-  cudaError_t le;
-  if (list_m == 64)
-    le = launch2_nks<2>(pipe, grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, est_rank, a_tile0, n_query, np, cand_score, cand_idx, stamps);
-  else
-    le = launch2_nks<4>(pipe, grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, est_rank, a_tile0, n_query, np, cand_score, cand_idx, stamps);
+  // SB2_KNN_SCAN=float keeps the float max tree in the fast path of the examination (same results, A/B timing)
+  const char* scan_env = getenv("SB2_KNN_SCAN");
+  const bool iscan = !(scan_env && strcmp(scan_env, "float") == 0);
+  const auto launch = list_m == 64 ? (iscan ? launch2_nks<2, true> : launch2_nks<2, false>)
+                                   : (iscan ? launch2_nks<4, true> : launch2_nks<4, false>);
+  const cudaError_t le =
+      launch(pipe, grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, est_rank, a_tile0, n_query, np, cand_score, cand_idx, stamps);
   SB2_CUDA(le);
   SB2_LAUNCH_CHECK(ctx);
   if (stamps) SB2_TRY(report_stamps(ctx, sh, pipe, grid, n_tiles + n_est, n_est, n_query, list_m, stamps));

@@ -1,11 +1,14 @@
-"""A/B of the kNN sweep's consumer loops on the bench workload's own X_pca (1.3M x 50, k = 15).
+"""A/B of the kNN sweep's consumer loops or of its fast paths on the bench workload's own X_pca (1.3M x 50, k = 15).
 
-PCA runs once; then SB2_KNN_PIPE=0 (single-buffer loop) and =1 (pipelined loop) alternate over --rounds rounds of
-_ops.knn_device.  Per setting: pass1_ms (CUDA events around the sweep launches), issued tensor TFLOP/s and, from one extra
-run with SB2_KNN_STAMPS=1, the split of the consumer warpgroups' cycles.  Asserts that (idx, dist) are bit-identical
-between the two settings.  Prints the card name and its power limit: the numbers mean nothing without them.
+PCA runs once; then the two settings of one switch alternate over --rounds rounds of _ops.knn_device:
+  --ab scan (default)  SB2_KNN_SCAN=float (float max tree in the fast path of the examination) against the default
+                       (integer maximum of the bit patterns)
+  --ab pipe            SB2_KNN_PIPE=0 (single-buffer loop) against =1 (pipelined loop)
+Per setting: pass1_ms (CUDA events around the sweep launches), issued tensor TFLOP/s and, from one extra run with
+SB2_KNN_STAMPS=1, the split of the consumer warpgroups' cycles.  Asserts that (idx, dist) are bit-identical between the
+two settings.  Prints the card name and its power limit: the numbers mean nothing without them.
 
-    python scripts/dev_knn_sweep.py [--n 1300000] [--rounds 5]
+    python scripts/dev_knn_sweep.py [--ab scan|pipe] [--n 1300000] [--rounds 5]
 """
 import argparse
 import os
@@ -55,6 +58,7 @@ def main():
     p.add_argument("--genes", type=int, default=2000)
     p.add_argument("--k", type=int, default=15)
     p.add_argument("--rounds", type=int, default=5)
+    p.add_argument("--ab", default="scan", choices=("scan", "pipe"), help="the switch whose two settings alternate")
     a = p.parse_args()
     print("card:", card(), flush=True)
     x, _ = synth_scipy(a.n, a.genes, device="cuda")
@@ -62,12 +66,13 @@ def main():
     ip, ix, dat = _ops.csr_to_device(x)
     xp = _ops.pca_csr_device(ctx, ip, ix, dat, a.n, a.genes, 50, solver=1)["X_pca"].contiguous()
     print(f"X_pca {tuple(xp.shape)}", flush=True)
-    settings = ("0", "1")
+    var, settings = {"scan": ("SB2_KNN_SCAN", ("float", "int")), "pipe": ("SB2_KNN_PIPE", ("0", "1"))}[a.ab]
+    old, new = settings
     ms = {s: [] for s in settings}
     ref = {}
     for r in range(a.rounds + 1):            # round 0 warms both settings up
         for s in settings:
-            os.environ["SB2_KNN_PIPE"] = s
+            os.environ[var] = s
             idx, dist, info = _ops.knn_device(ctx, xp, a.k)
             torch.cuda.synchronize()
             if r == 0:
@@ -75,24 +80,24 @@ def main():
                 continue
             ms[s].append(info["pass1_ms"])
             issued = info["pass1_issued_flops"] / (info["pass1_ms"] * 1e-3) / 1e12
-            print(f"round {r} PIPE={s}: pass1 {info['pass1_ms']:.1f} ms, issued {issued:.0f} TFLOP/s, "
+            print(f"round {r} {var}={s}: pass1 {info['pass1_ms']:.1f} ms, issued {issued:.0f} TFLOP/s, "
                   f"uncertified {info['n_uncertified']}, resweep {info['n_resweep']}", flush=True)
-    (i0, d0, f0), (i1, d1, f1) = ref["0"], ref["1"]
+    (i0, d0, f0), (i1, d1, f1) = ref[old], ref[new]
     same = bool(torch.equal(i0, i1) and torch.equal(d0, d1))
-    print(f"(idx, dist) bit-identical between PIPE=0 and PIPE=1: {same}; uncertified {f0['n_uncertified']} / {f1['n_uncertified']}, "
-          f"resweep {f0['n_resweep']} / {f1['n_resweep']}", flush=True)
+    print(f"(idx, dist) bit-identical between {var}={old} and {var}={new}: {same}; uncertified {f0['n_uncertified']} / "
+          f"{f1['n_uncertified']}, resweep {f0['n_resweep']} / {f1['n_resweep']}", flush=True)
     for s in settings:
         v = np.array(ms[s])
-        print(f"PIPE={s}: pass1_ms median {np.median(v):.1f} min {v.min():.1f} max {v.max():.1f} over {len(v)} rounds", flush=True)
-    print(f"pass1 median ratio new/old {np.median(ms['1']) / np.median(ms['0']):.3f}; slowest new {max(ms['1']):.1f} ms vs "
-          f"fastest old {min(ms['0']):.1f} ms", flush=True)
+        print(f"{var}={s}: pass1_ms median {np.median(v):.1f} min {v.min():.1f} max {v.max():.1f} over {len(v)} rounds", flush=True)
+    print(f"pass1 median ratio new/old {np.median(ms[new]) / np.median(ms[old]):.3f}; slowest new {max(ms[new]):.1f} ms vs "
+          f"fastest old {min(ms[old]):.1f} ms", flush=True)
     for s in settings:
-        os.environ["SB2_KNN_PIPE"] = s
+        os.environ[var] = s
         for ln in stamped(ctx, xp, a.k):
-            print(f"PIPE={s} {ln}", flush=True)
-    os.environ.pop("SB2_KNN_PIPE", None)
+            print(f"{var}={s} {ln}", flush=True)
+    os.environ.pop(var, None)
     print("card:", card(), flush=True)
-    assert same, "PIPE=0 and PIPE=1 disagree"
+    assert same, f"{var}={old} and {var}={new} disagree"
     assert (f0["n_uncertified"], f0["n_resweep"]) == (f1["n_uncertified"], f1["n_resweep"])
 
 
