@@ -31,11 +31,11 @@ from scipy import sparse
 
 from . import _abi, _ops
 from ._abi import check, ptr
-from ._compat import logger, settings
+from ._compat import logger
 from ._regress import _col_sums_stats
 
 MAX_COVARIATES = 32  # design columns besides the batch columns (sb2_regress_col_sums' weighted mode)
-TILE = 1024  # SB2_COMBAT_TILE_ROWS
+TILE = _ops.SUBTILE_ROWS  # SB2_COMBAT_TILE_ROWS
 PARTIAL_BYTES = 1 << 28  # device scratch for the moments' per-subtile partials
 
 
@@ -182,7 +182,7 @@ def eb_fit(counts, means, m2, b_hat_batch, grand_mean):
 
 
 # ------------------------------------------------------------------------------------------ device passes
-def _moments(dx: _ops.DeviceX, x, g: int, codes: np.ndarray, n_batch: int, cov: np.ndarray, grand, beta):
+def _moments(dx: _ops.DeviceX, g: int, codes: np.ndarray, n_batch: int, cov: np.ndarray, grand, beta):
     """(mean, M2) of r per batch [n_batch x g] each.  Each batch's rows go through in blocks of whole subtiles, so the
     result does not depend on the block size."""
     import torch
@@ -195,19 +195,12 @@ def _moments(dx: _ops.DeviceX, x, g: int, codes: np.ndarray, n_batch: int, cov: 
     d_cov = _ops._to_device(np.ascontiguousarray(cov[order])) if p else None
     d_grand = _ops._to_device(np.ascontiguousarray(grand, dtype=np.float64))
     d_beta = _ops._to_device(np.ascontiguousarray(beta, dtype=np.float64)) if p else None
-    subtiles = max(1, PARTIAL_BYTES // (2 * g * 8))
-    if dx.dense is not None:
-        subtiles = min(subtiles, max(1, settings.chunk_size // TILE))
-    step = subtiles * TILE
+    step = _ops.subtile_block_rows(dx.dense is not None, PARTIAL_BYTES, 2 * g * 8)
     accs = torch.zeros((n_batch, 3, g), dtype=torch.float64, device="cuda")
     for b in range(n_batch):
         for k0 in range(int(bounds[b]), int(bounds[b + 1]), step):
             k1 = min(int(bounds[b + 1]), k0 + step)
-            if dx.dense is None:
-                d_x, d_indptr, d_indices, d_data, d_ord = None, dx.indptr, dx.indices, dx.data, d_order[k0:k1]
-            else:
-                d_x = _ops._to_device(np.ascontiguousarray(x[order[k0:k1]], dtype=dx.dtype))
-                d_indptr = d_indices = d_data = d_ord = None
+            d_x, d_indptr, d_indices, d_data, d_ord = dx.gather(order, d_order, k0, k1)
             check(ctx.lib.sb2_combat_moments(ctx.handle, k1 - k0, g, dx.is_f64, ptr(d_x), ptr(d_indptr),
                                              ptr(d_indices), ptr(d_data), ptr(d_ord),
                                              ptr(d_cov[k0:] if p else None), p, ptr(d_grand), ptr(d_beta),
@@ -217,27 +210,21 @@ def _moments(dx: _ops.DeviceX, x, g: int, codes: np.ndarray, n_batch: int, cov: 
 
 
 def _adjust(dx: _ops.DeviceX, n: int, g: int, codes, cov, grand, beta, sqrt_vp, gamma_star, dsq) -> np.ndarray:
-    """The corrected float64 matrix, `settings.chunk_size` rows at a time, each block copied to the host before the
-    next."""
-    import torch
-
+    """The corrected float64 matrix (`_ops.write_dense`)."""
     ctx = _abi.default_context()
-    out = np.empty((n, g), dtype=np.float64)
     p = cov.shape[1]
     up = lambda a, dt: _ops._to_device(np.ascontiguousarray(a, dtype=dt))  # noqa: E731
     d_codes, d_grand, d_sv = up(codes, np.int32), up(grand, np.float64), up(sqrt_vp, np.float64)
     d_gamma, d_dsq = up(gamma_star, np.float64), up(dsq, np.float64)
     d_cov, d_beta = (up(cov, np.float64), up(beta, np.float64)) if p else (None, None)
-    step = max(1, int(settings.chunk_size))
-    for r0 in range(0, n, step):
-        r1 = min(n, r0 + step)
-        d_x, d_indptr, d_indices, d_data = dx.block(r0, r1)
-        d_out = torch.empty((r1 - r0, g), dtype=torch.float64, device="cuda")
+
+    def launch(r0, r1, xargs, d_out):
+        d_x, d_indptr, d_indices, d_data = xargs
         check(ctx.lib.sb2_combat_adjust(ctx.handle, r1 - r0, g, dx.is_f64, ptr(d_x), ptr(d_indptr), ptr(d_indices),
                                         ptr(d_data), ptr(d_codes[r0:]), ptr(d_cov[r0:] if p else None), p,
                                         ptr(d_grand), ptr(d_beta), ptr(d_sv), ptr(d_gamma), ptr(d_dsq), ptr(d_out)))
-        out[r0:r1] = _ops._to_host(d_out)
-    return out
+
+    return _ops.write_dense(dx, n, g, np.dtype(np.float64), launch)
 
 
 # ------------------------------------------------------------------------------------------ combat
@@ -277,7 +264,7 @@ def combat(adata, key: str = "batch", *, covariates=None, inplace: bool = True):
     grand_mean = np.dot((counts / float(counts.sum())).T, b_hat[:n_batch, :])
     beta = b_hat[n_batch:]
 
-    means, m2 = _moments(dx, x, g, codes, n_batch, cov, grand_mean, beta)
+    means, m2 = _moments(dx, g, codes, n_batch, cov, grand_mean, beta)
     fit = eb_fit(counts, means, m2, b_hat[:n_batch], grand_mean)
     logger.info("Adjusting data\n")
     res = _adjust(dx, n, g, codes, cov, grand_mean, beta, np.sqrt(fit["var_pooled"]), fit["gamma_star"],

@@ -137,6 +137,46 @@ class DeviceX:
             return None, self.indptr[r0:], self.indices, self.data
         return _to_device(np.ascontiguousarray(self.dense[r0:r1], dtype=self.dtype)), None, None, None
 
+    def gather(self, order: np.ndarray, d_order, k0: int, k1: int):
+        """The X arguments for call rows [k0, k1) of `order` (call row k is X row order[k]; `d_order` is `order` as int64
+        on the device, used with a CSR) -> (d_x, d_indptr, d_indices, d_data, d_order)."""
+        if self.dense is None:
+            return None, self.indptr, self.indices, self.data, d_order[k0:k1]
+        return _to_device(np.ascontiguousarray(self.dense[order[k0:k1]], dtype=self.dtype)), None, None, None, None
+
+
+SUBTILE_ROWS = 1024  # SB2_*_TILE_ROWS: the row subtile of the passes whose sums must not depend on the block size
+
+
+def subtile_block_rows(dense: bool, scratch_bytes: int, subtile_bytes: int) -> int:
+    """Rows per call of a subtiled pass: whole subtiles, so the sums do not depend on the block size, as many as the
+    partials' scratch holds (`subtile_bytes` per subtile) and, for a dense X, at most `settings.chunk_size` rows."""
+    from ._compat import settings
+
+    subtiles = max(1, scratch_bytes // subtile_bytes)
+    if dense:
+        subtiles = min(subtiles, max(1, settings.chunk_size // SUBTILE_ROWS))
+    return subtiles * SUBTILE_ROWS
+
+
+def write_dense(dx: DeviceX, n: int, g: int, out_dtype: np.dtype, launch) -> np.ndarray:
+    """The dense n x g result of a pass, `settings.chunk_size` rows at a time: `launch(r0, r1, (d_x, d_indptr,
+    d_indices, d_data), d_out)` fills the block's device output, which is copied into the host array before the next
+    block, so device memory does not grow with n x g."""
+    from ._compat import settings
+
+    torch = _torch()
+    out = np.empty((n, g), dtype=out_dtype)
+    tdt = torch.float64 if out_dtype == np.float64 else torch.float32
+    step = max(1, int(settings.chunk_size))
+    for r0 in range(0, n, step):
+        r1 = min(n, r0 + step)
+        xargs = dx.block(r0, r1)
+        d_out = torch.empty((r1 - r0, g), dtype=tdt, device="cuda")
+        launch(r0, r1, xargs, d_out)
+        out[r0:r1] = _to_host(d_out)
+    return out
+
 
 # ------------------------------------------------------------------------------------------ PCA
 def _pca_call(entry, ctx, args, n_rows, g: int, n_comps: int, *, mean: bool = True, extra=()):

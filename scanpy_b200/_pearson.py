@@ -31,7 +31,6 @@ from ._abi import check, ptr
 from ._compat import accepts_legacy_random_state, is_anndata_like, log_done, log_start, logger, settings, warn
 from ._regress import _col_sums
 
-TILE = 1024  # SB2_PEARSON_TILE_ROWS: the residual variance's fixed row subtile
 PARTIAL_BYTES = 1 << 28  # device scratch for the residual variance's per-subtile partials
 _DEFAULT = object()
 
@@ -89,7 +88,7 @@ def _totals(dx: _ops.DeviceX, n: int, g: int, codes: np.ndarray, n_batches: int)
     return gene, _row_sums(dx, n, g)
 
 
-def _residual_variances(dx: _ops.DeviceX, x, g: int, rows: np.ndarray, d_rows, d_cells, gene: np.ndarray,
+def _residual_variances(dx: _ops.DeviceX, g: int, rows: np.ndarray, d_rows, d_cells, gene: np.ndarray,
                         total: float, clip: float, theta: float):
     """(population variance of the clipped residuals, Σx²) per gene over the cells `rows` of one batch.  The rows go
     through in blocks of whole subtiles, so the result does not depend on the block size."""
@@ -98,19 +97,11 @@ def _residual_variances(dx: _ops.DeviceX, x, g: int, rows: np.ndarray, d_rows, d
     ctx = _abi.default_context()
     acc = torch.zeros(4 * g, dtype=torch.float64, device="cuda")
     d_gene = _ops._to_device(np.ascontiguousarray(gene, dtype=np.float64))
-    subtiles = max(1, PARTIAL_BYTES // (3 * g * 8))
-    if dx.dense is not None:
-        subtiles = min(subtiles, max(1, settings.chunk_size // TILE))
-    step = subtiles * TILE
+    step = _ops.subtile_block_rows(dx.dense is not None, PARTIAL_BYTES, 3 * g * 8)
     m = len(rows)
     for k0 in range(0, m, step):
         k1 = min(m, k0 + step)
-        if dx.dense is None:
-            d_x, d_indptr, d_indices, d_data = None, dx.indptr, dx.indices, dx.data
-            d_order = d_rows[k0:k1]
-        else:
-            d_x = _ops._to_device(np.ascontiguousarray(x[rows[k0:k1]], dtype=dx.dtype))
-            d_indptr = d_indices = d_data = d_order = None
+        d_x, d_indptr, d_indices, d_data, d_order = dx.gather(rows, d_rows, k0, k1)
         check(ctx.lib.sb2_pearson_residual_var(ctx.handle, k1 - k0, g, dx.is_f64, ptr(d_x), ptr(d_indptr),
                                                ptr(d_indices), ptr(d_data), ptr(d_order), ptr(d_gene),
                                                ptr(d_cells[k0:k1]), float(total), float(clip), float(theta), ptr(acc)))
@@ -167,7 +158,7 @@ def _highly_variable_pearson_residuals(adata, *, theta, clip, n_top_genes, batch
         if clip is None:
             clip = np.sqrt(k1 - k0)
         sum_total = np.sum(gene_tot[b][nonzero_genes])
-        var, sq_b = _residual_variances(dx, x, g, order[k0:k1], d_order[k0:k1] if d_order is not None else None,
+        var, sq_b = _residual_variances(dx, g, order[k0:k1], d_order[k0:k1] if d_order is not None else None,
                                         d_cells[k0:k1], gene_tot[b], sum_total, clip, theta)
         sq += sq_b
         residual_gene_vars.append(np.where(nonzero_genes, var, 0.0).reshape(1, -1))
@@ -261,26 +252,19 @@ def _pearson_residuals(x, theta, clip, check_values) -> np.ndarray:
     if check_values and not check_nonnegative_integers(x):
         warn("`normalize_pearson_residuals()` expects raw count data, but non-integers were found.", UserWarning)
 
-    import torch
-
     ctx = _abi.default_context()
     dx = _ops.DeviceX(x.tocsr() if sparse.issparse(x) else x, vdtype)
     gene_tot, d_cell = _totals(dx, n, g, np.zeros(n, dtype=np.int32), 1)
     sum_total = float(np.sum(gene_tot[0]))
     d_gene = _ops._to_device(np.ascontiguousarray(gene_tot[0]))
-    out_dtype = vdtype
-    out = np.empty((n, g), dtype=out_dtype)
-    tdt = torch.float64 if out_dtype == np.float64 else torch.float32
-    step = max(1, int(settings.chunk_size))
-    for r0 in range(0, n, step):
-        r1 = min(n, r0 + step)
-        d_x, d_indptr, d_indices, d_data = dx.block(r0, r1)
-        d_out = torch.empty((r1 - r0, g), dtype=tdt, device="cuda")
+
+    def launch(r0, r1, xargs, d_out):
+        d_x, d_indptr, d_indices, d_data = xargs
         check(ctx.lib.sb2_pearson_residuals(ctx.handle, r1 - r0, g, dx.is_f64, ptr(d_x), ptr(d_indptr),
                                             ptr(d_indices), ptr(d_data), ptr(d_gene), ptr(d_cell[r0:r1]), sum_total,
-                                            float(clip), float(theta), int(out_dtype == np.float64), ptr(d_out)))
-        out[r0:r1] = _ops._to_host(d_out)
-    return out
+                                            float(clip), float(theta), int(vdtype == np.float64), ptr(d_out)))
+
+    return _ops.write_dense(dx, n, g, vdtype, launch)
 
 
 def normalize_pearson_residuals(adata, *, theta: float = 100, clip: float | None = None, check_values: bool = True,

@@ -27,10 +27,10 @@ from scipy import sparse
 
 from . import _abi, _ops
 from ._abi import check, ptr
-from ._compat import log_done, log_start, logger, settings
+from ._compat import log_done, log_start, logger
 
 MAX_REGRESSORS = 32  # the intercept included
-TILE = 1024  # SB2_REGRESS_TILE_ROWS: the column sums' fixed row subtile
+TILE = _ops.SUBTILE_ROWS  # SB2_REGRESS_TILE_ROWS: the column sums' fixed row subtile
 PARTIAL_BYTES = 1 << 28  # device scratch for the column sums' per-subtile partials
 
 
@@ -69,12 +69,7 @@ def _col_sums_stats(dx: _DeviceX, n: int, g: int, *, w=None, group=None, n_group
     cmax = torch.full((g,), -np.inf, dtype=torch.float64, device="cuda")
     cnan = torch.zeros(g, dtype=torch.int32, device="cuda")
     d_w = _ops._to_device(np.ascontiguousarray(w, dtype=np.float64)) if w is not None else None
-    # blocks are whole subtiles (so the sums do not depend on the block size), bounded by the partials' scratch and,
-    # for a dense X, by settings.chunk_size
-    subtiles = max(1, PARTIAL_BYTES // ((width + 3) * g * 8))
-    if dx.dense is not None:
-        subtiles = min(subtiles, max(1, settings.chunk_size // TILE))
-    step = subtiles * TILE
+    step = _ops.subtile_block_rows(dx.dense is not None, PARTIAL_BYTES, (width + 3) * g * 8)
     for r0 in range(0, n, step):
         r1 = min(n, r0 + step)
         d_x, d_indptr, d_indices, d_data = dx.block(r0, r1)
@@ -93,27 +88,21 @@ def _col_sums_stats(dx: _DeviceX, n: int, g: int, *, w=None, group=None, n_group
 
 def _residual(dx: _DeviceX, n: int, g: int, out_dtype: np.dtype, *, w=None, coef=None, codes=None, means=None, b0=None,
               b1=None, passthrough=None) -> np.ndarray:
-    """The dense result, `settings.chunk_size` rows at a time, each block copied to the host before the next."""
-    import torch
-
+    """The dense result (`_ops.write_dense`)."""
     ctx = _abi.default_context()
-    out = np.empty((n, g), dtype=out_dtype)
     up = lambda a, dt: None if a is None else _ops._to_device(np.ascontiguousarray(a, dtype=dt))  # noqa: E731
     d_w, d_coef, d_codes, d_means = up(w, np.float64), up(coef, np.float64), up(codes, np.int32), up(means, np.float64)
     d_b0, d_b1, d_pass = up(b0, np.float64), up(b1, np.float64), up(passthrough, np.uint8)
-    tdt = torch.float64 if out_dtype == np.float64 else torch.float32
-    step = max(1, int(settings.chunk_size))
-    for r0 in range(0, n, step):
-        r1 = min(n, r0 + step)
-        d_x, d_indptr, d_indices, d_data = dx.block(r0, r1)
-        d_out = torch.empty((r1 - r0, g), dtype=tdt, device="cuda")
+
+    def launch(r0, r1, xargs, d_out):
+        d_x, d_indptr, d_indices, d_data = xargs
         check(ctx.lib.sb2_regress_residual(
             ctx.handle, r1 - r0, g, dx.is_f64, ptr(d_x), ptr(d_indptr), ptr(d_indices), ptr(d_data),
             ptr(d_w[r0:] if d_w is not None else None), coef.shape[0] if coef is not None else 0, ptr(d_coef),
             ptr(d_codes[r0:] if d_codes is not None else None), ptr(d_means), ptr(d_b0), ptr(d_b1), ptr(d_pass),
             int(out_dtype == np.float64), ptr(d_out)))
-        out[r0:r1] = _ops._to_host(d_out)
-    return out
+
+    return _ops.write_dense(dx, n, g, out_dtype, launch)
 
 
 def _categorical_fit(sums: np.ndarray, counts: np.ndarray, n: int, has_missing: bool):

@@ -8,7 +8,7 @@
 // shared-memory tile (slab.cuh).  All arithmetic is fp64.
 //
 // Moments: the count, mean and M2 (sum of squared deviations) of r over the rows of one batch.  One CTA per
-// (CB_TILE-row subtile, slab) accumulates shifted sums (shift = the subtile's first r) and writes the subtile's (mean,
+// (SLAB_TILE-row subtile, slab) accumulates shifted sums (shift = the subtile's first r) and writes the subtile's (mean,
 // M2); the subtiles are then merged into the caller's accumulators with Chan's formula in subtile order.  The caller
 // passes one batch at a time in blocks that start on a subtile boundary of the batch, so results are bit-identical
 // across runs and block sizes.  From these the host derives the pooled variance, gamma_hat, delta_hat and every sum of
@@ -23,9 +23,7 @@
 
 namespace {
 
-constexpr int CB_TILE = SB2_COMBAT_TILE_ROWS;
 constexpr int CB_MAXP = 32;
-static_assert(CB_TILE % SLAB_ROWS == 0, "subtile");
 
 // sum_k cov[k] * beta[k], then + grand: the order of `grand_mean + np.dot(tmp, b_hat)`
 template <int KMAX>
@@ -50,7 +48,7 @@ moments_kernel(int64_t rows, int g, const T* __restrict__ x, const int64_t* __re
   const int64_t sub = blockIdx.x;
   const int c0 = blockIdx.y * SLAB_THREADS, c = c0 + threadIdx.x;
   const int c1 = min(g, c0 + SLAB_THREADS);
-  const int64_t s0 = sub * CB_TILE, s1 = min(rows, s0 + CB_TILE);
+  const int64_t s0 = sub * SLAB_TILE, s1 = min(rows, s0 + SLAB_TILE);
   double bk[KMAX];
 #pragma unroll
   for (int k = 0; k < KMAX; ++k) bk[k] = (c < g && k < p) ? beta[(int64_t)k * g + c] : 0.0;
@@ -88,31 +86,6 @@ moments_kernel(int64_t rows, int g, const T* __restrict__ x, const int64_t* __re
   out[g + c] = a2 - a1 * a1 / m;
 }
 
-// acc[k][j] (k = 0 count, 1 mean, 2 M2) merged with the subtiles' partials in subtile order (Chan et al.)
-__global__ void moments_fold_kernel(int64_t nsub, int64_t rows, int g, const double* __restrict__ part,
-                                    double* __restrict__ acc) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= g) return;
-  double n = acc[j], mean = acc[g + j], m2 = acc[2 * (int64_t)g + j];
-  for (int64_t t = 0; t < nsub; ++t) {
-    const double* p = part + t * 2 * (int64_t)g;
-    const double nb = (double)min((int64_t)CB_TILE, rows - t * CB_TILE);
-    const double mb = p[j], m2b = p[g + j];
-    if (n == 0.0) {
-      mean = mb;
-      m2 = m2b;
-    } else {
-      const double nn = n + nb, d = mb - mean;
-      mean += d * (nb / nn);
-      m2 += m2b + d * d * (n * nb / nn);
-    }
-    n += nb;
-  }
-  acc[j] = n;
-  acc[g + j] = mean;
-  acc[2 * (int64_t)g + j] = m2;
-}
-
 // grid (row tiles of SLAB_ROWS, slabs)
 template <typename T, bool CSR, int KMAX>
 __global__ void __launch_bounds__(SLAB_THREADS)
@@ -147,35 +120,6 @@ adjust_kernel(int64_t rows, int g, const T* __restrict__ x, const int64_t* __res
   }
 }
 
-template <typename T, bool CSR>
-void launch_moments(sb2_ctx* ctx, dim3 grid, int64_t rows, int g, const void* x, const int64_t* indptr,
-                    const int32_t* indices, const void* data, const int64_t* order, const double* cov, int p,
-                    const double* grand, const double* beta, double* part) {
-  auto* xt = static_cast<const T*>(x);
-  auto* dt = static_cast<const T*>(data);
-  if (p > 4)
-    moments_kernel<T, CSR, CB_MAXP><<<grid, SLAB_THREADS, 0, ctx->stream>>>(rows, g, xt, indptr, indices, dt, order,
-                                                                           cov, p, grand, beta, part);
-  else
-    moments_kernel<T, CSR, 4><<<grid, SLAB_THREADS, 0, ctx->stream>>>(rows, g, xt, indptr, indices, dt, order, cov, p,
-                                                                     grand, beta, part);
-}
-
-template <typename T, bool CSR>
-void launch_adjust(sb2_ctx* ctx, dim3 grid, int64_t rows, int g, const void* x, const int64_t* indptr,
-                   const int32_t* indices, const void* data, const int32_t* batch, const double* cov, int p,
-                   const double* grand, const double* beta, const double* sqrt_vp, const double* gamma,
-                   const double* dsq, double* out) {
-  auto* xt = static_cast<const T*>(x);
-  auto* dt = static_cast<const T*>(data);
-  if (p > 4)
-    adjust_kernel<T, CSR, CB_MAXP><<<grid, SLAB_THREADS, 0, ctx->stream>>>(
-        rows, g, xt, indptr, indices, dt, batch, cov, p, grand, beta, sqrt_vp, gamma, dsq, out);
-  else
-    adjust_kernel<T, CSR, 4><<<grid, SLAB_THREADS, 0, ctx->stream>>>(rows, g, xt, indptr, indices, dt, batch, cov, p,
-                                                                    grand, beta, sqrt_vp, gamma, dsq, out);
-}
-
 }  // namespace
 
 extern "C" {
@@ -189,25 +133,22 @@ int32_t sb2_combat_moments(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f64
   SB2_CHECK_ARG(p >= 0 && p <= CB_MAXP && (p == 0 || (d_cov && d_beta)), "covariates");
   SB2_CUDA(cudaSetDevice(ctx->device));
   if (rows == 0) return SB2_OK;
-  const int64_t nsub = ceil_div64(rows, CB_TILE), slabs = ceil_div64(g, SLAB_THREADS);
+  const int64_t nsub = ceil_div64(rows, SLAB_TILE), slabs = ceil_div64(g, SLAB_THREADS);
   SB2_CHECK_ARG(nsub < INT32_MAX && slabs <= 65535, "shape");
   ScratchScope scr(ctx);
   double* part;
   SB2_TRY(scr.alloc(&part, (size_t)(nsub * 2 * g)));
   const dim3 grid((unsigned)nsub, (unsigned)slabs);
-  if (d_x) {
-    if (is_f64) launch_moments<double, false>(ctx, grid, rows, g, d_x, nullptr, nullptr, nullptr, d_order, d_cov, p,
-                                              d_grand, d_beta, part);
-    else launch_moments<float, false>(ctx, grid, rows, g, d_x, nullptr, nullptr, nullptr, d_order, d_cov, p, d_grand,
-                                      d_beta, part);
-  } else {
-    if (is_f64) launch_moments<double, true>(ctx, grid, rows, g, nullptr, d_indptr, d_indices, d_data, d_order, d_cov,
-                                             p, d_grand, d_beta, part);
-    else launch_moments<float, true>(ctx, grid, rows, g, nullptr, d_indptr, d_indices, d_data, d_order, d_cov, p,
-                                     d_grand, d_beta, part);
-  }
+  with_types(is_f64, d_x, [&](auto t, auto csr) {
+    using T = decltype(t);
+    with_kmax(p > 4, [&](auto kmax) {
+      moments_kernel<T, decltype(csr)::value, kmax><<<grid, SLAB_THREADS, 0, ctx->stream>>>(
+          rows, g, static_cast<const T*>(d_x), d_indptr, d_indices, static_cast<const T*>(d_data), d_order, d_cov, p,
+          d_grand, d_beta, part);
+    });
+  });
   SB2_LAUNCH_CHECK(ctx);
-  moments_fold_kernel<<<(unsigned)ceil_div64(g, 256), 256, 0, ctx->stream>>>(nsub, rows, g, part, d_acc);
+  moments_fold_kernel<false><<<(unsigned)ceil_div64(g, 256), 256, 0, ctx->stream>>>(nsub, rows, g, part, d_acc);
   SB2_LAUNCH_CHECK(ctx);
   return SB2_OK;
 }
@@ -226,17 +167,14 @@ int32_t sb2_combat_adjust(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f64,
   const int64_t tiles = ceil_div64(rows, SLAB_ROWS), slabs = ceil_div64(g, SLAB_THREADS);
   SB2_CHECK_ARG(tiles < INT32_MAX && slabs <= 65535, "shape");
   const dim3 grid((unsigned)tiles, (unsigned)slabs);
-  if (d_x) {
-    if (is_f64) launch_adjust<double, false>(ctx, grid, rows, g, d_x, nullptr, nullptr, nullptr, d_batch, d_cov, p,
-                                             d_grand, d_beta, d_sqrt_vp, d_gamma, d_dsq, d_out);
-    else launch_adjust<float, false>(ctx, grid, rows, g, d_x, nullptr, nullptr, nullptr, d_batch, d_cov, p, d_grand,
-                                     d_beta, d_sqrt_vp, d_gamma, d_dsq, d_out);
-  } else {
-    if (is_f64) launch_adjust<double, true>(ctx, grid, rows, g, nullptr, d_indptr, d_indices, d_data, d_batch, d_cov,
-                                            p, d_grand, d_beta, d_sqrt_vp, d_gamma, d_dsq, d_out);
-    else launch_adjust<float, true>(ctx, grid, rows, g, nullptr, d_indptr, d_indices, d_data, d_batch, d_cov, p,
-                                    d_grand, d_beta, d_sqrt_vp, d_gamma, d_dsq, d_out);
-  }
+  with_types(is_f64, d_x, [&](auto t, auto csr) {
+    using T = decltype(t);
+    with_kmax(p > 4, [&](auto kmax) {
+      adjust_kernel<T, decltype(csr)::value, kmax><<<grid, SLAB_THREADS, 0, ctx->stream>>>(
+          rows, g, static_cast<const T*>(d_x), d_indptr, d_indices, static_cast<const T*>(d_data), d_batch, d_cov, p,
+          d_grand, d_beta, d_sqrt_vp, d_gamma, d_dsq, d_out);
+    });
+  });
   SB2_LAUNCH_CHECK(ctx);
   return SB2_OK;
 }

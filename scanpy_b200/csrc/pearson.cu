@@ -10,7 +10,7 @@
 //
 // Row totals: one warp per row, a fixed-order lane-strided sum and a butterfly reduction.
 //
-// Residual variance: the population variance of r over the rows of one batch.  One CTA per (PR_TILE-row subtile,
+// Residual variance: the population variance of r over the rows of one batch.  One CTA per (SLAB_TILE-row subtile,
 // slab) accumulates shifted sums (shift = the subtile's first residual) and writes the subtile's (mean, M2); the
 // per-gene Σx² rides along.  The subtiles are then merged into the caller's accumulators with Chan's formula in subtile
 // order.  The caller passes one batch at a time in blocks that start on a subtile boundary of the batch, so results
@@ -26,9 +26,6 @@
 #include "slab.cuh"
 
 namespace {
-
-constexpr int PR_TILE = SB2_PEARSON_TILE_ROWS;
-static_assert(PR_TILE % SLAB_ROWS == 0, "subtile");
 
 __device__ __forceinline__ double pearson_residual(double v, double sg, double sc, double total, double clip,
                                                    double theta) {
@@ -70,7 +67,7 @@ resvar_kernel(int64_t rows, int g, const T* __restrict__ x, const int64_t* __res
   const int64_t sub = blockIdx.x;
   const int c0 = blockIdx.y * SLAB_THREADS, c = c0 + threadIdx.x;
   const int c1 = min(g, c0 + SLAB_THREADS);
-  const int64_t s0 = sub * PR_TILE, s1 = min(rows, s0 + PR_TILE);
+  const int64_t s0 = sub * SLAB_TILE, s1 = min(rows, s0 + SLAB_TILE);
   const double sg = c < g ? gene[c] : 0.0;
   double shift = 0.0, a1 = 0.0, a2 = 0.0, sq = 0.0;
   if (CSR)
@@ -110,33 +107,6 @@ resvar_kernel(int64_t rows, int g, const T* __restrict__ x, const int64_t* __res
   out[2 * (int64_t)g + c] = sq;
 }
 
-// acc[k][j] (k = 0 count, 1 mean, 2 M2, 3 Σx²) merged with the subtiles' partials in subtile order (Chan et al.)
-__global__ void resvar_fold_kernel(int64_t nsub, int64_t rows, int g, const double* __restrict__ part,
-                                   double* __restrict__ acc) {
-  const int j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= g) return;
-  double n = acc[j], mean = acc[g + j], m2 = acc[2 * (int64_t)g + j], sq = acc[3 * (int64_t)g + j];
-  for (int64_t t = 0; t < nsub; ++t) {
-    const double* p = part + t * 3 * (int64_t)g;
-    const double nb = (double)min((int64_t)PR_TILE, rows - t * PR_TILE);
-    const double mb = p[j], m2b = p[g + j];
-    if (n == 0.0) {
-      mean = mb;
-      m2 = m2b;
-    } else {
-      const double nn = n + nb, d = mb - mean;
-      mean += d * (nb / nn);
-      m2 += m2b + d * d * (n * nb / nn);
-    }
-    n += nb;
-    sq += p[2 * (int64_t)g + j];
-  }
-  acc[j] = n;
-  acc[g + j] = mean;
-  acc[2 * (int64_t)g + j] = m2;
-  acc[3 * (int64_t)g + j] = sq;
-}
-
 // grid (row tiles of SLAB_ROWS, slabs)
 template <typename T, typename O, bool CSR>
 __global__ void __launch_bounds__(SLAB_THREADS, 4)
@@ -173,24 +143,6 @@ void launch_row_sums(sb2_ctx* ctx, int64_t rows, int g, const void* x, const int
                                                                   static_cast<const T*>(data), out);
 }
 
-template <typename T, bool CSR>
-void launch_resvar(sb2_ctx* ctx, dim3 grid, int64_t rows, int g, const void* x, const int64_t* indptr,
-                   const int32_t* indices, const void* data, const int64_t* order, const double* gene,
-                   const double* cell, double total, double clip, double theta, double* part) {
-  resvar_kernel<T, CSR><<<grid, SLAB_THREADS, 0, ctx->stream>>>(rows, g, static_cast<const T*>(x), indptr, indices,
-                                                                 static_cast<const T*>(data), order, gene, cell, total,
-                                                                 clip, theta, part);
-}
-
-template <typename T, typename O, bool CSR>
-void launch_residual(sb2_ctx* ctx, dim3 grid, int64_t rows, int g, const void* x, const int64_t* indptr,
-                     const int32_t* indices, const void* data, const double* gene, const double* cell, double total,
-                     double clip, double theta, void* out) {
-  residual_kernel<T, O, CSR><<<grid, SLAB_THREADS, 0, ctx->stream>>>(rows, g, static_cast<const T*>(x), indptr,
-                                                                      indices, static_cast<const T*>(data), gene, cell,
-                                                                      total, clip, theta, static_cast<O*>(out));
-}
-
 }  // namespace
 
 extern "C" {
@@ -217,25 +169,20 @@ int32_t sb2_pearson_residual_var(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t 
   SB2_CHECK_ARG(theta > 0 && clip >= 0, "theta > 0, clip >= 0");
   SB2_CUDA(cudaSetDevice(ctx->device));
   if (rows == 0) return SB2_OK;
-  const int64_t nsub = ceil_div64(rows, PR_TILE), slabs = ceil_div64(g, SLAB_THREADS);
+  const int64_t nsub = ceil_div64(rows, SLAB_TILE), slabs = ceil_div64(g, SLAB_THREADS);
   SB2_CHECK_ARG(nsub < INT32_MAX && slabs <= 65535, "shape");
   ScratchScope scr(ctx);
   double* part;
   SB2_TRY(scr.alloc(&part, (size_t)(nsub * 3 * g)));
   const dim3 grid((unsigned)nsub, (unsigned)slabs);
-  if (d_x) {
-    if (is_f64) launch_resvar<double, false>(ctx, grid, rows, g, d_x, nullptr, nullptr, nullptr, d_order, d_gene, d_cell,
-                                             total, clip, theta, part);
-    else launch_resvar<float, false>(ctx, grid, rows, g, d_x, nullptr, nullptr, nullptr, d_order, d_gene, d_cell, total,
-                                     clip, theta, part);
-  } else {
-    if (is_f64) launch_resvar<double, true>(ctx, grid, rows, g, nullptr, d_indptr, d_indices, d_data, d_order, d_gene,
-                                            d_cell, total, clip, theta, part);
-    else launch_resvar<float, true>(ctx, grid, rows, g, nullptr, d_indptr, d_indices, d_data, d_order, d_gene, d_cell,
-                                    total, clip, theta, part);
-  }
+  with_types(is_f64, d_x, [&](auto t, auto csr) {
+    using T = decltype(t);
+    resvar_kernel<T, decltype(csr)::value><<<grid, SLAB_THREADS, 0, ctx->stream>>>(
+        rows, g, static_cast<const T*>(d_x), d_indptr, d_indices, static_cast<const T*>(d_data), d_order, d_gene, d_cell,
+        total, clip, theta, part);
+  });
   SB2_LAUNCH_CHECK(ctx);
-  resvar_fold_kernel<<<(unsigned)ceil_div64(g, 256), 256, 0, ctx->stream>>>(nsub, rows, g, part, d_acc);
+  moments_fold_kernel<true><<<(unsigned)ceil_div64(g, 256), 256, 0, ctx->stream>>>(nsub, rows, g, part, d_acc);
   SB2_LAUNCH_CHECK(ctx);
   return SB2_OK;
 }
@@ -253,18 +200,13 @@ int32_t sb2_pearson_residuals(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_
   const int64_t tiles = ceil_div64(rows, SLAB_ROWS), slabs = ceil_div64(g, SLAB_THREADS);
   SB2_CHECK_ARG(tiles < INT32_MAX && slabs <= 65535, "shape");
   const dim3 grid((unsigned)tiles, (unsigned)slabs);
-  const bool csr = d_x == nullptr;
-#define SB2_PEARSON(T, O, C)                                                                                  \
-  launch_residual<T, O, C>(ctx, grid, rows, g, d_x, d_indptr, d_indices, d_data, d_gene, d_cell, total, clip, \
-                           theta, d_out)
-  if (is_f64) {
-    if (csr) SB2_PEARSON(double, double, true); else SB2_PEARSON(double, double, false);
-  } else if (out_f64) {
-    if (csr) SB2_PEARSON(float, double, true); else SB2_PEARSON(float, double, false);
-  } else {
-    if (csr) SB2_PEARSON(float, float, true); else SB2_PEARSON(float, float, false);
-  }
-#undef SB2_PEARSON
+  with_types(is_f64, out_f64, d_x, [&](auto t, auto o, auto csr) {
+    using T = decltype(t);
+    using O = decltype(o);
+    residual_kernel<T, O, decltype(csr)::value><<<grid, SLAB_THREADS, 0, ctx->stream>>>(
+        rows, g, static_cast<const T*>(d_x), d_indptr, d_indices, static_cast<const T*>(d_data), d_gene, d_cell, total,
+        clip, theta, static_cast<O*>(d_out));
+  });
   SB2_LAUNCH_CHECK(ctx);
   return SB2_OK;
 }

@@ -4,10 +4,10 @@
 // Pass 1 (column sums): for every gene j, acc[k, j] = sum_i W[i, k] x[i, j] (weighted: W = the regressors A for the
 // numpy shortcut, or an orthonormal basis Q of range(A) for the GLM fallback), or acc[c, j] = sum of x[i, j] over the
 // rows of group c (categorical), plus the per-gene min / max / NaN flag that decide `not (col != col[0]).any()`.
-// One CTA owns a 256-column slab of a fixed RG_TILE-row subtile and each thread one column; it walks the subtile's rows
+// One CTA owns a 256-column slab of a fixed SLAB_TILE-row subtile and each thread one column; it walks the subtile's rows
 // in a fixed order (by group, then by row), so every partial is a sequential fp64 sum.  The subtiles' partials are
 // then folded into the accumulators in subtile order.  Sums therefore do not depend on the launch shape or on how the
-// caller splits the rows into blocks, as long as every block but the last is a multiple of RG_TILE rows: results are
+// caller splits the rows into blocks, as long as every block but the last is a multiple of SLAB_TILE rows: results are
 // bit-identical across runs and chunk sizes.
 //
 // Pass 2 (residual): out[i, j] = x[i, j] - fit[i, j] computed in fp64 and rounded once to the output type, with
@@ -23,26 +23,22 @@
 
 namespace {
 
-constexpr int RG_THREADS = SLAB_THREADS;
-constexpr int RG_ROWS = SLAB_ROWS;
-constexpr int RG_TILE = SB2_REGRESS_TILE_ROWS;
 constexpr int RG_MAXP = 32;
-static_assert(RG_TILE % RG_ROWS == 0, "subtile");
 
 // grid (subtiles, slabs).  Weighted (w != NULL): part[sub][k][j], k < p.  Categorical: part[sub][group][j], the groups a
 // subtile lacks stay as the caller zeroed them; `order` lists each subtile's rows sorted by (group, row).
 template <typename T, bool CSR, int KMAX>
-__global__ void __launch_bounds__(RG_THREADS)
+__global__ void __launch_bounds__(SLAB_THREADS)
 col_sums_kernel(int64_t rows, int g, const T* __restrict__ x, const int64_t* __restrict__ indptr,
                 const int32_t* __restrict__ indices, const T* __restrict__ data, const double* __restrict__ w, int p,
                 const int32_t* __restrict__ group, const int32_t* __restrict__ order, int n_groups,
                 double* __restrict__ part, double* __restrict__ pmin, double* __restrict__ pmax, int32_t* __restrict__ pnan) {
-  __shared__ T tile[CSR ? RG_ROWS : 1][RG_THREADS];
-  __shared__ int64_t rid[RG_ROWS], lo[RG_ROWS], hi[RG_ROWS];
+  __shared__ T tile[CSR ? SLAB_ROWS : 1][SLAB_THREADS];
+  __shared__ int64_t rid[SLAB_ROWS], lo[SLAB_ROWS], hi[SLAB_ROWS];
   const int64_t sub = blockIdx.x;
-  const int c0 = blockIdx.y * RG_THREADS, c = c0 + threadIdx.x;
-  const int c1 = min(g, c0 + RG_THREADS);
-  const int64_t s0 = sub * RG_TILE, s1 = min(rows, s0 + RG_TILE);
+  const int c0 = blockIdx.y * SLAB_THREADS, c = c0 + threadIdx.x;
+  const int c1 = min(g, c0 + SLAB_THREADS);
+  const int64_t s0 = sub * SLAB_TILE, s1 = min(rows, s0 + SLAB_TILE);
   const int64_t width = (int64_t)(w ? p : n_groups) * g;
   double* out = part + sub * width;
   double acc[KMAX];
@@ -52,9 +48,9 @@ col_sums_kernel(int64_t rows, int g, const T* __restrict__ x, const int64_t* __r
   int32_t nan = 0;
   int cur = -1;
   if (CSR)
-    for (int r = 0; r < RG_ROWS; ++r) tile[r][threadIdx.x] = T(0);
-  for (int64_t b = s0; b < s1; b += RG_ROWS) {
-    const int m = (int)min((int64_t)RG_ROWS, s1 - b);
+    for (int r = 0; r < SLAB_ROWS; ++r) tile[r][threadIdx.x] = T(0);
+  for (int64_t b = s0; b < s1; b += SLAB_ROWS) {
+    const int m = (int)min((int64_t)SLAB_ROWS, s1 - b);
     if (CSR) {
       if ((int)threadIdx.x < m) rid[threadIdx.x] = order ? order[b + threadIdx.x] : b + threadIdx.x;
       stage_csr(indptr, indices, data, rid, m, c0, c1, tile, lo, hi);
@@ -128,22 +124,22 @@ __global__ void fold_kernel(int64_t nsub, int64_t width, int g, const double* __
   }
 }
 
-// grid (row tiles of RG_ROWS, slabs)
+// grid (row tiles of SLAB_ROWS, slabs)
 template <typename T, typename O, bool CSR, int KMAX>
-__global__ void __launch_bounds__(RG_THREADS)
+__global__ void __launch_bounds__(SLAB_THREADS)
 residual_kernel(int64_t rows, int g, const T* __restrict__ x, const int64_t* __restrict__ indptr,
                 const int32_t* __restrict__ indices, const T* __restrict__ data, const double* __restrict__ w, int p,
                 const double* __restrict__ coef, const int32_t* __restrict__ code, const double* __restrict__ means,
                 const double* __restrict__ b0, const double* __restrict__ b1, const uint8_t* __restrict__ pass,
                 O* __restrict__ out) {
-  __shared__ T tile[CSR ? RG_ROWS : 1][RG_THREADS];
-  __shared__ int64_t rid[RG_ROWS], lo[RG_ROWS], hi[RG_ROWS];
-  const int64_t r0 = (int64_t)blockIdx.x * RG_ROWS;
-  const int m = (int)min((int64_t)RG_ROWS, rows - r0);
-  const int c0 = blockIdx.y * RG_THREADS, c = c0 + threadIdx.x;
-  const int c1 = min(g, c0 + RG_THREADS);
+  __shared__ T tile[CSR ? SLAB_ROWS : 1][SLAB_THREADS];
+  __shared__ int64_t rid[SLAB_ROWS], lo[SLAB_ROWS], hi[SLAB_ROWS];
+  const int64_t r0 = (int64_t)blockIdx.x * SLAB_ROWS;
+  const int m = (int)min((int64_t)SLAB_ROWS, rows - r0);
+  const int c0 = blockIdx.y * SLAB_THREADS, c = c0 + threadIdx.x;
+  const int c1 = min(g, c0 + SLAB_THREADS);
   if (CSR) {
-    for (int r = 0; r < RG_ROWS; ++r) tile[r][threadIdx.x] = T(0);
+    for (int r = 0; r < SLAB_ROWS; ++r) tile[r][threadIdx.x] = T(0);
     if ((int)threadIdx.x < m) rid[threadIdx.x] = r0 + threadIdx.x;
     stage_csr(indptr, indices, data, rid, m, c0, c1, tile, lo, hi);
   }
@@ -176,35 +172,6 @@ residual_kernel(int64_t rows, int g, const T* __restrict__ x, const int64_t* __r
   }
 }
 
-template <typename T, bool CSR>
-void launch_col_sums(sb2_ctx* ctx, dim3 grid, int64_t rows, int g, const void* x, const int64_t* indptr,
-                     const int32_t* indices, const void* data, const double* w, int p, const int32_t* group,
-                     const int32_t* order, int n_groups, double* part, double* pmin, double* pmax, int32_t* pnan) {
-  auto* xt = static_cast<const T*>(x);
-  auto* dt = static_cast<const T*>(data);
-  if (w && p > 4)
-    col_sums_kernel<T, CSR, RG_MAXP><<<grid, RG_THREADS, 0, ctx->stream>>>(rows, g, xt, indptr, indices, dt, w, p, group,
-                                                                          order, n_groups, part, pmin, pmax, pnan);
-  else
-    col_sums_kernel<T, CSR, 4><<<grid, RG_THREADS, 0, ctx->stream>>>(rows, g, xt, indptr, indices, dt, w, p, group,
-                                                                    order, n_groups, part, pmin, pmax, pnan);
-}
-
-template <typename T, typename O, bool CSR>
-void launch_residual(sb2_ctx* ctx, dim3 grid, int64_t rows, int g, const void* x, const int64_t* indptr,
-                     const int32_t* indices, const void* data, const double* w, int p, const double* coef,
-                     const int32_t* code, const double* means, const double* b0, const double* b1, const uint8_t* pass,
-                     void* out) {
-  auto* xt = static_cast<const T*>(x);
-  auto* dt = static_cast<const T*>(data);
-  if (w && p > 4)
-    residual_kernel<T, O, CSR, RG_MAXP><<<grid, RG_THREADS, 0, ctx->stream>>>(
-        rows, g, xt, indptr, indices, dt, w, p, coef, code, means, b0, b1, pass, static_cast<O*>(out));
-  else
-    residual_kernel<T, O, CSR, 4><<<grid, RG_THREADS, 0, ctx->stream>>>(
-        rows, g, xt, indptr, indices, dt, w, p, coef, code, means, b0, b1, pass, static_cast<O*>(out));
-}
-
 }  // namespace
 
 extern "C" {
@@ -218,7 +185,7 @@ int32_t sb2_regress_col_sums(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f
   SB2_CHECK_ARG(d_w ? (p >= 1 && p <= RG_MAXP) : (d_group && d_order && n_groups >= 1), "weights or groups");
   SB2_CUDA(cudaSetDevice(ctx->device));
   if (rows == 0) return SB2_OK;
-  const int64_t nsub = ceil_div64(rows, RG_TILE), slabs = ceil_div64(g, RG_THREADS);
+  const int64_t nsub = ceil_div64(rows, SLAB_TILE), slabs = ceil_div64(g, SLAB_THREADS);
   SB2_CHECK_ARG(nsub < INT32_MAX && slabs <= 65535, "shape");
   const int64_t width = (int64_t)(d_w ? p : n_groups) * g;
   ScratchScope scr(ctx);
@@ -232,17 +199,14 @@ int32_t sb2_regress_col_sums(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f
   const dim3 grid((unsigned)nsub, (unsigned)slabs);
   const int32_t* order = d_w ? nullptr : d_order;
   const int32_t* group = d_w ? nullptr : d_group;
-  if (d_x) {
-    if (is_f64) launch_col_sums<double, false>(ctx, grid, rows, g, d_x, nullptr, nullptr, nullptr, d_w, p, group, order,
-                                               n_groups, part, pmin, pmax, pnan);
-    else launch_col_sums<float, false>(ctx, grid, rows, g, d_x, nullptr, nullptr, nullptr, d_w, p, group, order,
-                                       n_groups, part, pmin, pmax, pnan);
-  } else {
-    if (is_f64) launch_col_sums<double, true>(ctx, grid, rows, g, nullptr, d_indptr, d_indices, d_data, d_w, p, group,
-                                              order, n_groups, part, pmin, pmax, pnan);
-    else launch_col_sums<float, true>(ctx, grid, rows, g, nullptr, d_indptr, d_indices, d_data, d_w, p, group, order,
-                                      n_groups, part, pmin, pmax, pnan);
-  }
+  with_types(is_f64, d_x, [&](auto t, auto csr) {
+    using T = decltype(t);
+    with_kmax(d_w && p > 4, [&](auto kmax) {
+      col_sums_kernel<T, decltype(csr)::value, kmax><<<grid, SLAB_THREADS, 0, ctx->stream>>>(
+          rows, g, static_cast<const T*>(d_x), d_indptr, d_indices, static_cast<const T*>(d_data), d_w, p, group, order,
+          n_groups, part, pmin, pmax, pnan);
+    });
+  });
   SB2_LAUNCH_CHECK(ctx);
   const int64_t span = width > g ? width : g;
   fold_kernel<<<(unsigned)ceil_div64(span, 256), 256, 0, ctx->stream>>>(nsub, width, g, part, pmin, pmax, pnan, d_acc,
@@ -262,21 +226,18 @@ int32_t sb2_regress_residual(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f
   SB2_CHECK_ARG(is_f64 ? out_f64 : 1, "a float64 X needs a float64 output");
   SB2_CUDA(cudaSetDevice(ctx->device));
   if (rows == 0) return SB2_OK;
-  const int64_t tiles = ceil_div64(rows, RG_ROWS), slabs = ceil_div64(g, RG_THREADS);
+  const int64_t tiles = ceil_div64(rows, SLAB_ROWS), slabs = ceil_div64(g, SLAB_THREADS);
   SB2_CHECK_ARG(tiles < INT32_MAX && slabs <= 65535, "shape");
   const dim3 grid((unsigned)tiles, (unsigned)slabs);
-  const bool csr = d_x == nullptr;
-#define SB2_RESIDUAL(T, O, C)                                                                                       \
-  launch_residual<T, O, C>(ctx, grid, rows, g, d_x, d_indptr, d_indices, d_data, d_w, p, d_coef, d_code, d_means, \
-                           d_b0, d_b1, d_pass, d_out)
-  if (is_f64) {
-    if (csr) SB2_RESIDUAL(double, double, true); else SB2_RESIDUAL(double, double, false);
-  } else if (out_f64) {
-    if (csr) SB2_RESIDUAL(float, double, true); else SB2_RESIDUAL(float, double, false);
-  } else {
-    if (csr) SB2_RESIDUAL(float, float, true); else SB2_RESIDUAL(float, float, false);
-  }
-#undef SB2_RESIDUAL
+  with_types(is_f64, out_f64, d_x, [&](auto t, auto o, auto csr) {
+    using T = decltype(t);
+    using O = decltype(o);
+    with_kmax(d_w && p > 4, [&](auto kmax) {
+      residual_kernel<T, O, decltype(csr)::value, kmax><<<grid, SLAB_THREADS, 0, ctx->stream>>>(
+          rows, g, static_cast<const T*>(d_x), d_indptr, d_indices, static_cast<const T*>(d_data), d_w, p, d_coef, d_code,
+          d_means, d_b0, d_b1, d_pass, static_cast<O*>(d_out));
+    });
+  });
   SB2_LAUNCH_CHECK(ctx);
   return SB2_OK;
 }
