@@ -142,17 +142,17 @@ int32_t sb2_tsvd_csr_f32(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_in
  *   pass 1: sb2_pca_stream_accumulate_f32 adds the chunk's column sums / sums of squares into d_stats fp64 [2g] and its
  *           X^T X into d_gram fp64 [g x g] (caller zero-fills both before the first chunk);
  *   solve : sb2_pca_stream_solve_f32 -> d_components [k x g], h_var, h_var_ratio, h_mean as sb2_pca_csr_f32, plus the
- *           projection operator d_proj fp32 [g x 128] (first g * *h_l entries used), d_shift fp32 [128], *h_l (32/64/128);
+ *           projection operator d_proj fp32 [g x 128] (first g * *h_l entries used), d_shift fp64 [128], *h_l (32/64/128);
  *   pass 2: sb2_pca_stream_project_f32 -> d_x_pca [n_chunk x k] = X_chunk U - mu^T U. */
 int32_t sb2_pca_stream_accumulate_f32(sb2_ctx* ctx, int64_t n_chunk, int32_t g, const int64_t* d_indptr,
                                       const int32_t* d_indices, const float* d_data, double* d_stats, double* d_gram);
 int32_t sb2_pca_stream_solve_f32(sb2_ctx* ctx, int64_t n_total, int32_t g, const double* d_stats, const double* d_gram,
                                  int32_t k, int32_t max_iter, double tol, uint64_t seed, float* d_components, double* h_var,
-                                 double* h_var_ratio, double* h_mean, float* d_proj, float* d_shift, int32_t* h_l,
+                                 double* h_var_ratio, double* h_mean, float* d_proj, double* d_shift, int32_t* h_l,
                                  sb2_pca_info* info);
 int32_t sb2_pca_stream_project_f32(sb2_ctx* ctx, int64_t n_chunk, int32_t g, const int64_t* d_indptr,
                                    const int32_t* d_indices, const float* d_data, int32_t k, int32_t l, const float* d_proj,
-                                   const float* d_shift, float* d_x_pca);
+                                   const double* d_shift, float* d_x_pca);
 
 /* ---- exact brute-force kNN (euclidean) -----------------------------------------------------
  * points: d_x [n_points x d] float32 row-major.  Queries are rows [q0, q0+n_query) of the same

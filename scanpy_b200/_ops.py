@@ -215,7 +215,7 @@ def _pca_stream_solve(ctx, n: int, g: int, stats, gram, n_comps: int, seed: int)
     -> (result dict with X_pca None, and the projection operator proj, shift, l for sb2_pca_stream_project_f32)."""
     torch = _torch()
     proj = torch.empty(g * 128, dtype=torch.float32, device="cuda")
-    shift = torch.empty(128, dtype=torch.float32, device="cuda")
+    shift = torch.empty(128, dtype=torch.float64, device="cuda")
     l = c_int32()
     out = _pca_call(ctx.lib.sb2_pca_stream_solve_f32, ctx, (n, g, ptr(stats), ptr(gram), n_comps, 0, 0.0, seed), None, g,
                     n_comps, extra=(ptr(proj), ptr(shift), byref(l)))

@@ -62,19 +62,21 @@ __global__ void reduce_copies_f32_to_f64_kernel(const float* __restrict__ src, i
 
 // ---------------------------------------------------------------------------------------------
 // Y[r, 0:ncols_out] = sum_e data[e] * B[indices[e], :] - shift     (row stride of Y = ldy)
-template <int LPT>  // columns of B per lane: l = 32*LPT
+// Acc = float for the passes of the iteration; Acc = double for the final projection X U - 1 (mu^T U), whose two terms
+// nearly cancel when genes have large means (fp32 products are exact in fp64, so only U's rounding remains)
+template <int LPT, typename Acc>  // columns of B per lane: l = 32*LPT
 __global__ void __launch_bounds__(256)
 spmm_csr_kernel(int64_t n, const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
-                const float* __restrict__ data, const float* __restrict__ B, const float* __restrict__ shift,
+                const float* __restrict__ data, const float* __restrict__ B, const Acc* __restrict__ shift,
                 float* __restrict__ Y, int ldy, int ncols_out) {
   constexpr int L = 32 * LPT;
   const int lane = threadIdx.x & 31;
   const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (row >= n) return;
   const int64_t e0 = indptr[row], e1 = indptr[row + 1];
-  float acc[LPT];
+  Acc acc[LPT];
 #pragma unroll
-  for (int j = 0; j < LPT; ++j) acc[j] = 0.0f;
+  for (int j = 0; j < LPT; ++j) acc[j] = Acc(0);
   for (int64_t e = e0; e < e1; e += 32) {
     const int cnt = (int)min((int64_t)32, e1 - e);
     int c = 0;
@@ -85,27 +87,27 @@ spmm_csr_kernel(int64_t n, const int64_t* __restrict__ indptr, const int32_t* __
     }
     for (int j = 0; j < cnt; ++j) {
       const int cj = __shfl_sync(0xffffffffu, c, j);
-      const float vj = __shfl_sync(0xffffffffu, v, j);
+      const Acc vj = __shfl_sync(0xffffffffu, v, j);
       const float* b = B + (size_t)cj * L + lane * LPT;
       if (LPT == 1) {
-        acc[0] = fmaf(vj, b[0], acc[0]);
+        acc[0] = fma(vj, (Acc)b[0], acc[0]);
       } else if (LPT == 2) {
         const float2 bb = *reinterpret_cast<const float2*>(b);
-        acc[0] = fmaf(vj, bb.x, acc[0]);
-        acc[1] = fmaf(vj, bb.y, acc[1]);
+        acc[0] = fma(vj, (Acc)bb.x, acc[0]);
+        acc[1] = fma(vj, (Acc)bb.y, acc[1]);
       } else {
         const float4 bb = *reinterpret_cast<const float4*>(b);
-        acc[0] = fmaf(vj, bb.x, acc[0]);
-        acc[1] = fmaf(vj, bb.y, acc[1]);
-        acc[2] = fmaf(vj, bb.z, acc[2]);
-        acc[3] = fmaf(vj, bb.w, acc[3]);
+        acc[0] = fma(vj, (Acc)bb.x, acc[0]);
+        acc[1] = fma(vj, (Acc)bb.y, acc[1]);
+        acc[2] = fma(vj, (Acc)bb.z, acc[2]);
+        acc[3] = fma(vj, (Acc)bb.w, acc[3]);
       }
     }
   }
 #pragma unroll
   for (int j = 0; j < LPT; ++j) {
     const int col = lane * LPT + j;
-    if (col < ncols_out) Y[row * (int64_t)ldy + col] = acc[j] - (shift ? shift[col] : 0.0f);
+    if (col < ncols_out) Y[row * (int64_t)ldy + col] = (float)(acc[j] - (shift ? shift[col] : Acc(0)));
   }
 }
 
@@ -649,6 +651,7 @@ struct PcaWork {
   // scratch
   float* d_Bf;      // [g x l] fp32 copy of a block V (the projection U at the end)
   float* d_shift;   // [l] mu^T V of that block
+  double* d_pshift; // [l] mu^T U of the projection U in d_Bf, in fp64 (see project_rows)
   double* d_S;      // [l x l]
   double* d_M;      // [l x l]
   double *d_Z, *d_tmp, *d_theta, *d_res;  // [g x l], [g x l], [l], [l]
@@ -656,18 +659,22 @@ struct PcaWork {
   // results
   double* d_V;                // [g x l] Ritz vectors, columns by descending Ritz value
   std::vector<double> theta;  // [l] Ritz values
-  double total_var0;          // sum of per-gene variances, ddof 0 (TruncatedSVD's ratio denominator)
+  std::vector<double> res;    // [l] their residual norms |A v - theta v|
+  double floor;               // tol * theta_0: the operator's rounding floor, below which a Ritz value is zero
+  double raw_over_centred;    // |X|_F^2 / |X_c|_F^2 (1 without centring): how far the fp32 SpMM passes cancel
+  double total_var0;         // sum of per-gene variances, ddof 0 (TruncatedSVD's ratio denominator)
   sb2_pca_info stats;         // loop statistics and the ddof-1 total variance
 };
 
+template <typename Acc>
 int32_t launch_spmm(sb2_ctx* ctx, int64_t n, int l, const int64_t* indptr, const int32_t* indices, const float* data,
-                    const float* B, const float* shift, float* Y, int ldy, int ncols_out) {
+                    const float* B, const Acc* shift, float* Y, int ldy, int ncols_out) {
   const int wpb = 8;
   const unsigned grid = (unsigned)ceil_div64(n, wpb);
   if (n == 0) return SB2_OK;
-  if (l == 32) spmm_csr_kernel<1><<<grid, wpb * 32, 0, ctx->stream>>>(n, indptr, indices, data, B, shift, Y, ldy, ncols_out);
-  else if (l == 64) spmm_csr_kernel<2><<<grid, wpb * 32, 0, ctx->stream>>>(n, indptr, indices, data, B, shift, Y, ldy, ncols_out);
-  else if (l == 128) spmm_csr_kernel<4><<<grid, wpb * 32, 0, ctx->stream>>>(n, indptr, indices, data, B, shift, Y, ldy, ncols_out);
+  if (l == 32) spmm_csr_kernel<1, Acc><<<grid, wpb * 32, 0, ctx->stream>>>(n, indptr, indices, data, B, shift, Y, ldy, ncols_out);
+  else if (l == 64) spmm_csr_kernel<2, Acc><<<grid, wpb * 32, 0, ctx->stream>>>(n, indptr, indices, data, B, shift, Y, ldy, ncols_out);
+  else if (l == 128) spmm_csr_kernel<4, Acc><<<grid, wpb * 32, 0, ctx->stream>>>(n, indptr, indices, data, B, shift, Y, ldy, ncols_out);
   else { sb2_set_error("spmm: l must be 32, 64 or 128 (got %d)", l); return SB2_E_BADARG; }
   SB2_LAUNCH_CHECK(ctx);
   return SB2_OK;
@@ -793,20 +800,21 @@ int32_t orthonormalize(PcaWork& w, double* A) {
   }
   return SB2_OK;
 }
-__global__ void mu_dot_kernel(const double* __restrict__ mu, const double* __restrict__ V, int g, int l,
-                              float* __restrict__ shift) {
+template <typename TV, typename TS>
+__global__ void mu_dot_kernel(const double* __restrict__ mu, const TV* __restrict__ V, int g, int l,
+                              TS* __restrict__ shift) {
   // one block per column j
   __shared__ double red[256];
   const int j = blockIdx.x;
   double s = 0.0;
-  for (int r = threadIdx.x; r < g; r += blockDim.x) s = fma(mu[r], V[(size_t)r * l + j], s);
+  for (int r = threadIdx.x; r < g; r += blockDim.x) s = fma(mu[r], (double)V[(size_t)r * l + j], s);
   red[threadIdx.x] = s;
   __syncthreads();
   for (int k = blockDim.x / 2; k > 0; k >>= 1) {
     if (threadIdx.x < k) red[threadIdx.x] += red[threadIdx.x + k];
     __syncthreads();
   }
-  if (threadIdx.x == 0) shift[j] = (float)red[0];
+  if (threadIdx.x == 0) shift[j] = (TS)red[0];
 }
 
 // Z = A_op * V  (V, Z device g x l fp64); A_op = X_c^T X_c summed over all ranks
@@ -829,7 +837,7 @@ int32_t apply_operator(PcaWork& w, const double* V, double* Z) {
   SB2_LAUNCH_CHECK(w.ctx);
   mu_dot_kernel<<<l, 256, 0, w.st>>>(w.d_mu, V, g, l, w.d_shift);
   SB2_LAUNCH_CHECK(w.ctx);
-  SB2_TRY(launch_spmm(w.ctx, w.n, l, w.indptr, w.indices, w.data, w.d_Bf, w.d_shift, w.d_Y, l, l));
+  SB2_TRY(launch_spmm<float>(w.ctx, w.n, l, w.indptr, w.indices, w.data, w.d_Bf, w.d_shift, w.d_Y, l, l));
   SB2_TRY(launch_spmm_t(w.ctx, w.n, g, l, w.indptr, w.indices, w.data, w.d_Y, w.d_Zc, Z));
   return sb2_comm_allreduce_f64(w.ctx, Z, len);
 }
@@ -873,12 +881,15 @@ int32_t gene_moments(PcaWork& w, const double* d_stats, double* h_mean) {
   SB2_CUDA(cudaMemcpyAsync(hs.data(), d_stats, sizeof(double) * 2 * g, cudaMemcpyDeviceToHost, w.st));
   SB2_CUDA(cudaStreamSynchronize(w.st));
   const double nt = (double)w.n_total;
+  double raw = 0.0;
   for (int j = 0; j < g; ++j) {
     const double mu = hs[j] / nt;
     h_mean[j] = mu;
     w.stats.total_var += (hs[g + j] - nt * mu * mu) / (nt - 1.0);  // per-gene variance, ddof=1 (_pca.py:727-729)
     w.total_var0 += hs[g + j] / nt - mu * mu;
+    raw += hs[g + j];
   }
+  w.raw_over_centred = w.total_var0 > 0.0 ? raw / (nt * w.total_var0) : 1.0;
   return SB2_OK;
 }
 // In-core entries: the gene moments of the CSR rows, column statistics summed over the ranks
@@ -972,6 +983,7 @@ int32_t subspace_iteration(PcaWork& w, ScratchScope& scr, int k, int max_iter, d
   std::vector<double> hres(l);
   std::vector<double>& theta = w.theta;
   theta.resize(l);
+  w.res.assign(l, 0.0);
   int32_t &it = w.stats.iterations, &converged = w.stats.converged;
   double& max_rel = w.stats.max_rel_residual;
   int stalled = 0;
@@ -1005,8 +1017,11 @@ int32_t subspace_iteration(PcaWork& w, ScratchScope& scr, int k, int max_iter, d
     SB2_CUDA(cudaStreamSynchronize(st));
     max_rel = 0.0;
     const double th1 = std::max(theta[0], 1e-300);
-    for (int j = 0; j < k; ++j) max_rel = std::max(max_rel, sqrt(std::max(hres[j], 0.0)) / th1);
-    converged = max_rel <= tol && theta[k - 1] > 0.0;
+    for (int j = 0; j < l; ++j) w.res[j] = sqrt(std::max(hres[j], 0.0));
+    for (int j = 0; j < k; ++j) max_rel = std::max(max_rel, w.res[j] / th1);
+    // A is PSD: a negative Ritz value is not converged unless it sits at the rounding floor (|theta| <= tol * theta_0), where
+    // a Ritz vector with a residual under tol * theta_0 is a null direction of A (centred rank below k), and exact
+    converged = max_rel <= tol && theta[k - 1] >= -tol * th1;
     if (max_rel <= goal && converged) break;
     if (it >= max_iter) break;
     // stagnation at the operator's rounding floor (fp32 SpMM passes): stop; converged iff under tol
@@ -1045,13 +1060,25 @@ int32_t subspace_iteration(PcaWork& w, ScratchScope& scr, int k, int max_iter, d
     }
     SB2_TRY(orthonormalize(w, d_V));
   }
+  // The SpMM passes centre in fp32 (X V - 1 mu^T V, then X^T of that), with rounding of about 2^-24 |X|_F^2 against an
+  // operator of norm <= |X_c|_F^2.  When gene means are large against their spread that exceeds the tolerance, and the
+  // residuals, measured on the same rounded operator, cannot certify the answer: it is never reported as converged.
+  if (w.solver == 0 && 0x1p-24 * w.raw_over_centred > tol) converged = 0;
+  w.floor = tol * std::max(theta[0], 0.0);
   return SB2_OK;
 }
 
+// |X|_F^2 / |X_c|_F^2 above which X_pca is projected in fp64.  The fp32 projection's rounding grows with the square root of
+// that ratio, because X U and 1 mu^T U nearly cancel when gene means are large against their spread.  Normalised
+// expression data sit near 1.2, where fp32 stays two orders of magnitude inside the 1e-4 bar; genes with means of
+// 100-1000 and unit spread reach 1e5, where fp32 misses the bar and fp64 (fp32 products are exact in it) does not.
+constexpr double PROJ_F64_RATIO = 4.0;
+
 // Signs of svd_flip(u_based_decision=False) (sklearn/utils/extmath.py:974-981) on the Ritz vectors w.d_V (in place), the
 // components d_components [k x g] (rows beyond g in the padded space are all-zero genes and are dropped), and the float32
-// projection operator of X_pca = X U - 1 (mu^T U): U [g x l] in w.d_Bf, mu^T U [l] in a fresh w.d_shift.
-int32_t projection_operator(PcaWork& w, ScratchScope& scr, int k, float* d_components) {
+// projection operator of X_pca = X U - 1 (mu^T U): U [g x l] in w.d_Bf, mu^T U [l] in w.d_shift (fp32, of the fp64 V) and
+// in w.d_pshift (fp64, of that fp32 U) when fp64_shift is set.
+int32_t projection_operator(PcaWork& w, ScratchScope& scr, int k, float* d_components, bool fp64_shift) {
   const int g = w.g_real, l = w.l;
   double *d_V = w.d_V, *d_am;
   SB2_TRY(scr.alloc(&d_am, (size_t)l));
@@ -1074,13 +1101,29 @@ int32_t projection_operator(PcaWork& w, ScratchScope& scr, int k, float* d_compo
   SB2_TRY(scr.alloc(&w.d_shift, (size_t)l));
   mu_dot_kernel<<<l, 256, 0, w.st>>>(w.d_mu, d_V, g, l, w.d_shift);
   SB2_LAUNCH_CHECK(w.ctx);
+  if (!fp64_shift) return SB2_OK;
+  SB2_TRY(scr.alloc(&w.d_pshift, (size_t)l));
+  mu_dot_kernel<<<l, 256, 0, w.st>>>(w.d_mu, w.d_Bf, g, l, w.d_pshift);
+  SB2_LAUNCH_CHECK(w.ctx);
   return SB2_OK;
 }
+
+// X_pca [n x k] = X U - 1 (mu^T U) of the in-core entries
+int32_t project_rows(const PcaWork& w, int64_t n, const int64_t* indptr, const int32_t* indices, const float* data, int k,
+                     float* d_x_pca) {
+  if (w.raw_over_centred > PROJ_F64_RATIO)
+    return launch_spmm<double>(w.ctx, n, w.l, indptr, indices, data, w.d_Bf, w.d_pshift, d_x_pca, k, k);
+  return launch_spmm<float>(w.ctx, n, w.l, indptr, indices, data, w.d_Bf, w.d_shift, d_x_pca, k, k);
+}
+
+// theta_j as an eigenvalue of the PSD operator: zero when it is within its own residual norm or the operator's rounding
+// floor of zero (a null direction whose Ritz value is rounding noise)
+double ritz_value(const PcaWork& w, int j) { return w.theta[j] <= std::max(w.res[j], w.floor) ? 0.0 : w.theta[j]; }
 
 // PCA: explained_variance_ = S^2/(n-1) (_pca.py:760-779), the ratio against the ddof-1 total
 void centred_variance(const PcaWork& w, int k, double* h_var, double* h_var_ratio) {
   for (int j = 0; j < k; ++j) {
-    const double ev = std::max(w.theta[j], 0.0) / ((double)w.n_total - 1.0);
+    const double ev = ritz_value(w, j) / ((double)w.n_total - 1.0);
     h_var[j] = ev;
     h_var_ratio[j] = w.stats.total_var > 0.0 ? ev / w.stats.total_var : 0.0;
   }
@@ -1095,7 +1138,7 @@ int32_t tsvd_variance(const PcaWork& w, int k, const double* h_mean, double* h_v
   for (int j = 0; j < k; ++j) {
     double m = 0.0;
     for (int r = 0; r < g; ++r) m += h_mean[r] * hV[(size_t)r * l + j];
-    const double ev = std::max(w.theta[j], 0.0) / (double)w.n_total - m * m;
+    const double ev = std::max(ritz_value(w, j) / (double)w.n_total - m * m, 0.0);
     h_var[j] = ev;
     h_var_ratio[j] = w.total_var0 > 0.0 ? ev / w.total_var0 : 0.0;
   }
@@ -1145,7 +1188,7 @@ int32_t sb2_spmm_csr(sb2_ctx* ctx, int64_t n, int32_t g, int32_t l, const int64_
                      const float* d_data, const float* d_b, const float* d_shift, float* d_y) {
   SB2_CHECK_ARG(ctx && d_indptr && d_b && d_y, "null pointer");
   SB2_CUDA(cudaSetDevice(ctx->device));
-  return launch_spmm(ctx, n, l, d_indptr, d_indices, d_data, d_b, d_shift, d_y, l, l);
+  return launch_spmm<float>(ctx, n, l, d_indptr, d_indices, d_data, d_b, d_shift, d_y, l, l);
 }
 
 int32_t sb2_spmm_csr_t(sb2_ctx* ctx, int64_t n, int32_t g, int32_t l, const int64_t* d_indptr,
@@ -1234,8 +1277,8 @@ int32_t sb2_pca_csr_f32(sb2_ctx* ctx, int64_t n, int64_t n_total, int32_t g, con
   SB2_CUDA(cudaMemcpyAsync(w.d_mu, h_mean, sizeof(double) * g, cudaMemcpyHostToDevice, w.st));
   SB2_TRY(incore_operator(w, scr, n, d_indptr, d_indices, d_data));
   SB2_TRY(subspace_iteration(w, scr, k, max_iter, tol, seed));
-  SB2_TRY(projection_operator(w, scr, k, d_components));
-  SB2_TRY(launch_spmm(ctx, n, w.l, d_indptr, d_indices, d_data, w.d_Bf, w.d_shift, d_x_pca, k, k));
+  SB2_TRY(projection_operator(w, scr, k, d_components, w.raw_over_centred > PROJ_F64_RATIO));
+  SB2_TRY(project_rows(w, n, d_indptr, d_indices, d_data, k, d_x_pca));
   centred_variance(w, k, h_var, h_var_ratio);
   return report(w, info);
 }
@@ -1256,10 +1299,11 @@ int32_t sb2_tsvd_csr_f32(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_in
   // the operator is X^T X itself: with an all-zero device mean neither the Gram centring nor the SpMM shift does anything;
   // the true column means stay on the host for the variance formula
   SB2_CUDA(cudaMemsetAsync(w.d_mu, 0, sizeof(double) * g, w.st));
+  w.raw_over_centred = 1.0;
   SB2_TRY(incore_operator(w, scr, n, d_indptr, d_indices, d_data));
   SB2_TRY(subspace_iteration(w, scr, k, max_iter, tol, seed));
-  SB2_TRY(projection_operator(w, scr, k, d_components));
-  SB2_TRY(launch_spmm(ctx, n, w.l, d_indptr, d_indices, d_data, w.d_Bf, w.d_shift, d_x_pca, k, k));
+  SB2_TRY(projection_operator(w, scr, k, d_components, w.raw_over_centred > PROJ_F64_RATIO));
+  SB2_TRY(project_rows(w, n, d_indptr, d_indices, d_data, k, d_x_pca));
   SB2_TRY(tsvd_variance(w, k, h_mean.data(), h_var, h_var_ratio));
   return report(w, info);
 }
@@ -1292,7 +1336,7 @@ int32_t sb2_pca_stream_accumulate_f32(sb2_ctx* ctx, int64_t n_chunk, int32_t g, 
 }
 int32_t sb2_pca_stream_solve_f32(sb2_ctx* ctx, int64_t n_total, int32_t g, const double* d_stats, const double* d_gram,
                                  int32_t k, int32_t max_iter, double tol, uint64_t seed, float* d_components, double* h_var,
-                                 double* h_var_ratio, double* h_mean, float* d_proj, float* d_shift, int32_t* h_l,
+                                 double* h_var_ratio, double* h_mean, float* d_proj, double* d_shift, int32_t* h_l,
                                  sb2_pca_info* info) {
   SB2_CHECK_ARG(ctx && d_stats && d_gram && d_components && h_var && h_var_ratio && h_mean && d_proj && d_shift && h_l,
                 "null pointer");
@@ -1304,20 +1348,20 @@ int32_t sb2_pca_stream_solve_f32(sb2_ctx* ctx, int64_t n_total, int32_t g, const
   SB2_CUDA(cudaMemcpyAsync(w.d_mu, h_mean, sizeof(double) * g, cudaMemcpyHostToDevice, w.st));
   SB2_TRY(gram_operator(w, scr, d_gram, false));
   SB2_TRY(subspace_iteration(w, scr, k, max_iter, tol, seed));
-  SB2_TRY(projection_operator(w, scr, k, d_components));
+  SB2_TRY(projection_operator(w, scr, k, d_components, true));
   SB2_CUDA(cudaMemcpyAsync(d_proj, w.d_Bf, sizeof(float) * (size_t)g * w.l, cudaMemcpyDeviceToDevice, w.st));
-  SB2_CUDA(cudaMemcpyAsync(d_shift, w.d_shift, sizeof(float) * w.l, cudaMemcpyDeviceToDevice, w.st));
+  SB2_CUDA(cudaMemcpyAsync(d_shift, w.d_pshift, sizeof(double) * w.l, cudaMemcpyDeviceToDevice, w.st));
   *h_l = w.l;
   centred_variance(w, k, h_var, h_var_ratio);
   return report(w, info);
 }
 int32_t sb2_pca_stream_project_f32(sb2_ctx* ctx, int64_t n_chunk, int32_t g, const int64_t* d_indptr,
                                    const int32_t* d_indices, const float* d_data, int32_t k, int32_t l, const float* d_proj,
-                                   const float* d_shift, float* d_x_pca) {
+                                   const double* d_shift, float* d_x_pca) {
   SB2_CHECK_ARG(ctx && d_indptr && d_proj && d_shift && d_x_pca, "null pointer");
   SB2_CHECK_ARG(k >= 1 && k <= l && (l == 32 || l == 64 || l == 128), "k / l");
   SB2_CUDA(cudaSetDevice(ctx->device));
-  return launch_spmm(ctx, n_chunk, l, d_indptr, d_indices, d_data, d_proj, d_shift, d_x_pca, k, k);
+  return launch_spmm<double>(ctx, n_chunk, l, d_indptr, d_indices, d_data, d_proj, d_shift, d_x_pca, k, k);
 }
 
 }  // extern "C"

@@ -108,6 +108,9 @@ def pca(data, n_comps: int | None = None, *, layer: str | None = None, obsm: str
         # sklearn's message for svd_solver='arpack' (pinned by tests/test_pca.py:292-296)
         raise ValueError(f"n_components={n_comps!r} must be between 1 and min(n_samples, n_features)="
                          f"{min(n_obs, n_vars)!r} with svd_solver='arpack'")
+    if n_comps > 120:
+        # the block iteration of csrc/pca.cu keeps n_comps + 8 vectors in a block of at most 128
+        raise NotImplementedError(f"scanpy_b200.pp.pca computes at most 120 components (n_comps={n_comps!r})")
     xc = x if backed else as_csr_f32(x)
     solver = _solver_code(svd_solver, n_vars=n_vars) if (zero_center and not chunked) else 1
     if not zero_center and not chunked:
