@@ -101,18 +101,29 @@ struct PhaseTimer {
 };
 
 #ifdef __CUDACC__
-__device__ __forceinline__ float warp_sum(float v) {
+template <typename T>
+__device__ __forceinline__ T warp_sum(T v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
+// sum over the CTA of one value per thread, in a fixed order (warp tree, then warps in order); result on thread 0
+template <typename T>
+__device__ __forceinline__ T block_sum(T v, T* red) {
+  v = warp_sum(v);
+  const int w = threadIdx.x >> 5;
+  if ((threadIdx.x & 31) == 0) red[w] = v;
+  __syncthreads();
+  T s = 0;
+  if (threadIdx.x == 0)
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += red[i];
+  __syncthreads();
+  return s;
 }
 #endif
 
 // ---- util.cu ----
 // out[0..n] (int64) = exclusive prefix sum of in[0..n) (int32 counts); out[n] = total
 int32_t sb2_scan_i32_to_i64(sb2_ctx* ctx, const int32_t* d_in, int64_t n, int64_t* d_out);
+// host cyclic Jacobi: A (m x m symmetric, row-major, destroyed) -> eigenvalues w, eigenvectors V (columns)
+void jacobi_eigh(std::vector<double>& A, int m, std::vector<double>& w, std::vector<double>& V);

@@ -42,7 +42,6 @@ eig_dots_kernel(int64_t n, int nv, const double* __restrict__ V, int64_t ld, con
                 double* __restrict__ partial) {
   __shared__ double red[8];
   const int64_t r0 = (int64_t)blockIdx.x * RB;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   double wv[RB / 256];
 #pragma unroll
   for (int j = 0; j < RB / 256; ++j) {
@@ -57,15 +56,8 @@ eig_dots_kernel(int64_t n, int nv, const double* __restrict__ V, int64_t ld, con
       const int64_t i = r0 + threadIdx.x + j * 256;
       if (i < n) acc += v[i] * wv[j];
     }
-    acc = warp_sum(acc);
-    if (lane == 0) red[warp] = acc;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double t = 0.0;
-      for (int k = 0; k < 8; ++k) t += red[k];
-      partial[(size_t)blockIdx.x * nv + c] = t;
-    }
-    __syncthreads();
+    const double t = block_sum(acc, red);
+    if (threadIdx.x == 0) partial[(size_t)blockIdx.x * nv + c] = t;
   }
 }
 // h[c] = sum_b partial[b][c]  (fixed order: deterministic); one warp per c
@@ -135,45 +127,6 @@ eig_transition_scale_kernel(int64_t n, const int64_t* __restrict__ indptr, const
     const double qi = 1.0 / q[row];
     out[row] = qi / sqrt(qi * acc);
   }
-}
-
-// cyclic Jacobi for a dense symmetric m x m matrix (row-major a, destroyed); eigenvalues -> d, eigenvectors -> columns of z
-void jacobi_eigh(int m, std::vector<double>& a, std::vector<double>& d, std::vector<double>& z) {
-  z.assign((size_t)m * m, 0.0);
-  for (int i = 0; i < m; ++i) z[(size_t)i * m + i] = 1.0;
-  for (int sweep = 0; sweep < 60; ++sweep) {
-    double off = 0.0, diag = 0.0;
-    for (int i = 0; i < m; ++i) {
-      diag += a[(size_t)i * m + i] * a[(size_t)i * m + i];
-      for (int j = i + 1; j < m; ++j) off += a[(size_t)i * m + j] * a[(size_t)i * m + j];
-    }
-    if (off <= 1e-30 * (diag + off) || off == 0.0) break;
-    for (int p = 0; p < m - 1; ++p)
-      for (int q = p + 1; q < m; ++q) {
-        const double apq = a[(size_t)p * m + q];
-        if (fabs(apq) < 1e-300) continue;
-        const double theta = (a[(size_t)q * m + q] - a[(size_t)p * m + p]) / (2.0 * apq);
-        const double t = (theta >= 0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-        for (int k = 0; k < m; ++k) {
-          const double akp = a[(size_t)k * m + p], akq = a[(size_t)k * m + q];
-          a[(size_t)k * m + p] = c * akp - s * akq;
-          a[(size_t)k * m + q] = s * akp + c * akq;
-        }
-        for (int k = 0; k < m; ++k) {
-          const double apk = a[(size_t)p * m + k], aqk = a[(size_t)q * m + k];
-          a[(size_t)p * m + k] = c * apk - s * aqk;
-          a[(size_t)q * m + k] = s * apk + c * aqk;
-        }
-        for (int k = 0; k < m; ++k) {
-          const double zkp = z[(size_t)k * m + p], zkq = z[(size_t)k * m + q];
-          z[(size_t)k * m + p] = c * zkp - s * zkq;
-          z[(size_t)k * m + q] = s * zkp + c * zkq;
-        }
-      }
-  }
-  d.resize(m);
-  for (int i = 0; i < m; ++i) d[i] = a[(size_t)i * m + i];
 }
 
 struct Eigs {
@@ -280,7 +233,7 @@ extern "C" int32_t sb2_eigsh_csr_scaled(sb2_ctx* ctx, int64_t n, const int64_t* 
     Tw.assign((size_t)me * me, 0.0);
     for (int i = 0; i < me; ++i)
       for (int j = 0; j < me; ++j) Tw[(size_t)i * me + j] = T[(size_t)i * m + j];
-    jacobi_eigh(me, Tw, theta, Y);   // Y: me x me, eigenvector i in column i
+    jacobi_eigh(Tw, me, theta, Y);   // Y: me x me, eigenvector i in column i
     order.resize(me);
     std::iota(order.begin(), order.end(), 0);
     auto key = [&](int i) { return which == 1 ? fabs(theta[i]) : which == 0 ? theta[i] : -theta[i]; };

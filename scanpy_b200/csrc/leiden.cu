@@ -92,16 +92,9 @@ __global__ void strength_kernel(int32_t n, const int64_t* __restrict__ indptr, c
     k[v] = s;
   }
   // block reduce -> one atomic
-  __shared__ long long red[8];
-  long long x = s;
-  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = x;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    long long t = 0;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
-    atomicAdd(total, (u64)t);
-  }
+  __shared__ int64_t red[8];
+  const int64_t t = block_sum(s, red);
+  if (threadIdx.x == 0) atomicAdd(total, (u64)t);
 }
 __global__ void comm_stats_kernel(int32_t n, const int32_t* __restrict__ comm, const int64_t* __restrict__ k,
                                   u64* __restrict__ K, int32_t* __restrict__ csize) {
@@ -392,7 +385,7 @@ agg_count_kernel(int32_t nc, const int64_t* __restrict__ slice, const int32_t* _
   if (r >= nc) return;
   int c = 0;
   for (int64_t s = slice[r] + lane; s < slice[r + 1]; s += 32) c += hkeys[s] >= 0;
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+  c = warp_sum(c);
   if (lane == 0) cnt[r] = c;
 }
 __global__ void __launch_bounds__(256)
@@ -425,7 +418,7 @@ agg_count_block_kernel(int32_t nc, const int64_t* __restrict__ slice, const int3
   __syncthreads();
   int c = 0;
   for (int64_t s = slice[r] + threadIdx.x; s < slice[r + 1]; s += blockDim.x) c += hkeys[s] >= 0;
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+  c = warp_sum(c);
   if ((threadIdx.x & 31) == 0 && c) atomicAdd(&total, c);
   __syncthreads();
   if (threadIdx.x == 0) cnt[r] = total;
@@ -469,7 +462,7 @@ __global__ void internal_weight_kernel(int32_t n, const int64_t* __restrict__ in
     for (int64_t e = indptr[v]; e < indptr[v + 1]; ++e)
       if (comm[indices[e]] == c) s += w[e];
   }
-  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  s = warp_sum(s);
   if ((threadIdx.x & 31) == 0 && s != 0) atomicAdd(internal, (u64)s);
 }
 __global__ void relabel_kernel(int64_t n, int32_t* __restrict__ comm, const int32_t* __restrict__ newid) {

@@ -5,9 +5,8 @@
 // and the `covariance_eigh` Gram route of src/scanpy/preprocessing/_pca/_dask.py:143-213 +
 // _pca/_kernels.py:14-58.
 //
-// Kernels (all HBM/L2-bound integer+fp32 streaming work; no tensor cores):
-//   csr_col_stats_kernel   one CSR pass: per-gene sum and sum of squares (fp64 REDs into replicated
-//                          accumulators)                                   bytes: 8*nnz + 8*(n+1)
+// Kernels (all HBM/L2-bound integer+fp32 streaming work; no tensor cores; the per-gene sum and sum of
+// squares are sb2_csr_col_sums_f32's one CSR pass in preprocess.cu):
 //   spmm_csr_kernel        Y = X*B - 1*shift^T, warp per row, lanes own l/32 columns of B;
 //                          coalesced column-index loads, shuffle-broadcast of (col,val), B rows are
 //                          read as one 128..512 B segment per non-zero     bytes: 8*nnz + 4*n*l
@@ -17,7 +16,7 @@
 //   small dense fp64 helpers (g x l blocks, l <= 128): A^T B, A*M, C*V, residual norms.
 //   rr_jacobi_kernel       the l x l Rayleigh-Ritz eigenproblem for l <= 64, one CTA (fp64).
 // Host side (C++ in this file): the block subspace iteration, CholeskyQR2 with an eigen-based
-// fallback for rank-deficient blocks, and a cyclic-Jacobi eigensolver for the l = 128 Rayleigh-Ritz
+// fallback for rank-deficient blocks; util.cu's cyclic-Jacobi eigensolver takes the l = 128 Rayleigh-Ritz
 // problem (fp64).  Centering never densifies X:  X_c B = X B - 1 (mu^T B) and, because
 // the columns of that product sum to zero, X_c^T (X_c B) = X^T (X B - 1 mu^T B).
 #include <math.h>
@@ -30,27 +29,9 @@
 
 namespace {
 
-constexpr int STAT_COPIES = 32;
 constexpr int ZT_COPIES = 8;
 
 // ---------------------------------------------------------------------------------------------
-__global__ void csr_col_stats_kernel(int64_t nnz, const int32_t* __restrict__ indices, const float* __restrict__ data,
-                                     int g, double* __restrict__ acc /* [COPIES][2][g] */) {
-  double* mine = acc + (size_t)(blockIdx.x % STAT_COPIES) * 2 * g;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nnz; i += (int64_t)gridDim.x * blockDim.x) {
-    const int c = indices[i];
-    const double v = data[i];
-    atomicAdd(&mine[c], v);
-    atomicAdd(&mine[g + c], v * v);
-  }
-}
-__global__ void reduce_copies_f64_kernel(const double* __restrict__ src, int copies, int64_t len, double* __restrict__ dst) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= len) return;
-  double s = 0.0;
-  for (int c = 0; c < copies; ++c) s += src[(size_t)c * len + i];
-  dst[i] = s;
-}
 __global__ void reduce_copies_f32_to_f64_kernel(const float* __restrict__ src, int copies, int64_t len,
                                                 double* __restrict__ dst) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -531,47 +512,6 @@ rr_jacobi_kernel(const double* __restrict__ S, int m, double* __restrict__ W, do
 
 // ---------------------------------------------------------------------------------------------
 // host fp64 small dense algebra
-// cyclic Jacobi: A (m x m symmetric, row-major, destroyed) -> eigenvalues w, eigenvectors V (columns)
-void jacobi_eigh(std::vector<double>& A, int m, std::vector<double>& w, std::vector<double>& V) {
-  V.assign((size_t)m * m, 0.0);
-  for (int i = 0; i < m; ++i) V[(size_t)i * m + i] = 1.0;
-  for (int sweep = 0; sweep < 60; ++sweep) {
-    double off = 0.0, diag = 0.0;
-    for (int i = 0; i < m; ++i) {
-      diag += A[(size_t)i * m + i] * A[(size_t)i * m + i];
-      for (int j = i + 1; j < m; ++j) off += A[(size_t)i * m + j] * A[(size_t)i * m + j];
-    }
-    if (off <= 1e-30 * (diag + off) || off == 0.0) break;
-    for (int p = 0; p < m - 1; ++p) {
-      for (int q = p + 1; q < m; ++q) {
-        const double apq = A[(size_t)p * m + q];
-        if (apq == 0.0) continue;
-        const double app = A[(size_t)p * m + p], aqq = A[(size_t)q * m + q];
-        if (fabs(apq) < 1e-300) continue;
-        const double tau = (aqq - app) / (2.0 * apq);
-        const double t = (tau >= 0.0 ? 1.0 : -1.0) / (fabs(tau) + sqrt(1.0 + tau * tau));
-        const double c = 1.0 / sqrt(1.0 + t * t), s = t * c;
-        for (int k = 0; k < m; ++k) {  // columns p,q
-          const double akp = A[(size_t)k * m + p], akq = A[(size_t)k * m + q];
-          A[(size_t)k * m + p] = c * akp - s * akq;
-          A[(size_t)k * m + q] = s * akp + c * akq;
-        }
-        for (int k = 0; k < m; ++k) {  // rows p,q
-          const double apk = A[(size_t)p * m + k], aqk = A[(size_t)q * m + k];
-          A[(size_t)p * m + k] = c * apk - s * aqk;
-          A[(size_t)q * m + k] = s * apk + c * aqk;
-        }
-        for (int k = 0; k < m; ++k) {
-          const double vkp = V[(size_t)k * m + p], vkq = V[(size_t)k * m + q];
-          V[(size_t)k * m + p] = c * vkp - s * vkq;
-          V[(size_t)k * m + q] = s * vkp + c * vkq;
-        }
-      }
-    }
-  }
-  w.resize(m);
-  for (int i = 0; i < m; ++i) w[i] = A[(size_t)i * m + i];
-}
 // sort eigenpairs descending
 void sort_desc(std::vector<double>& w, std::vector<double>& V, int m) {
   std::vector<int> ord(m);
@@ -1161,27 +1101,12 @@ int32_t sb2_csr_col_stats(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_i
   SB2_CHECK_ARG(ctx && d_indptr && d_col_sum && d_col_sumsq, "null pointer");
   SB2_CHECK_ARG(n >= 0 && g >= 1, "shape");
   SB2_CUDA(cudaSetDevice(ctx->device));
-  ScratchScope scr(ctx);
   int64_t nnz = 0;
   if (n > 0) {
     SB2_CUDA(cudaMemcpyAsync(&nnz, d_indptr + n, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
     SB2_CUDA(cudaStreamSynchronize(ctx->stream));
   }
-  double* acc;
-  SB2_TRY(scr.alloc(&acc, (size_t)STAT_COPIES * 2 * g));
-  SB2_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * STAT_COPIES * 2 * g, ctx->stream));
-  if (nnz > 0) {
-    const int grid = ctx->prop.multiProcessorCount * 8;
-    csr_col_stats_kernel<<<grid, 256, 0, ctx->stream>>>(nnz, d_indices, d_data, g, acc);
-    SB2_LAUNCH_CHECK(ctx);
-  }
-  double* both;
-  SB2_TRY(scr.alloc(&both, (size_t)2 * g));
-  reduce_copies_f64_kernel<<<(unsigned)ceil_div64(2 * g, 256), 256, 0, ctx->stream>>>(acc, STAT_COPIES, 2 * (int64_t)g, both);
-  SB2_LAUNCH_CHECK(ctx);
-  SB2_CUDA(cudaMemcpyAsync(d_col_sum, both, sizeof(double) * g, cudaMemcpyDeviceToDevice, ctx->stream));
-  SB2_CUDA(cudaMemcpyAsync(d_col_sumsq, both + g, sizeof(double) * g, cudaMemcpyDeviceToDevice, ctx->stream));
-  return SB2_OK;
+  return sb2_csr_col_sums_f32(ctx, nnz, g, d_indices, d_data, 0, 1.0, d_col_sum, d_col_sumsq);
 }
 
 int32_t sb2_spmm_csr(sb2_ctx* ctx, int64_t n, int32_t g, int32_t l, const int64_t* d_indptr, const int32_t* d_indices,

@@ -53,14 +53,15 @@ __global__ void log1p_kernel(int64_t nnz, float* __restrict__ data, double log_b
   if (log_base != 0.0) v = (float)((double)v / log_base);  // np.divide(x, np.log(base)) (_simple.py:359-380)
   data[i] = v;
 }
-// per-gene sum and sum of squares of f(x), f = expm1(x * log_scale) or identity; fp64 REDs into replicated copies
+// per-gene sum and sum of squares of f(x), f = expm1(x * log_scale) (EXPM1) or identity; fp64 REDs into replicated copies
 constexpr int MV_COPIES = 32;
+template <bool EXPM1>
 __global__ void col_sums_transformed_kernel(int64_t nnz, const int32_t* __restrict__ indices, const float* __restrict__ data,
-                                            int g, int apply_expm1, float log_scale, double* __restrict__ acc) {
+                                            int g, double* __restrict__ acc, float log_scale) {
   double* mine = acc + (size_t)(blockIdx.x % MV_COPIES) * 2 * g;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nnz; i += (int64_t)gridDim.x * blockDim.x) {
     float x = data[i];
-    if (apply_expm1) {
+    if (EXPM1) {
       if (log_scale != 1.0f) x *= log_scale;
       x = expm1f(x);
     }
@@ -171,6 +172,21 @@ __global__ void dense_scale_kernel(int64_t n, int g, T* __restrict__ x, const do
 
 inline unsigned gridw(int64_t n) { return (unsigned)ceil_div64(n, 8); }
 
+// zeroed [MV_COPIES][2][g] accumulators for the column-stats kernels, and the [2][g] buffer finish_col_stats sums them into
+int32_t alloc_col_stats(sb2_ctx* ctx, ScratchScope& scr, int32_t g, double** acc, double** both) {
+  SB2_TRY(scr.alloc(acc, (size_t)MV_COPIES * 2 * g));
+  SB2_TRY(scr.alloc(both, (size_t)2 * g));
+  SB2_CUDA(cudaMemsetAsync(*acc, 0, sizeof(double) * MV_COPIES * 2 * g, ctx->stream));
+  return SB2_OK;
+}
+int32_t finish_col_stats(sb2_ctx* ctx, const double* acc, double* both, int32_t g, double* d_sum, double* d_sumsq) {
+  reduce_copies_kernel<<<(unsigned)ceil_div64(2 * g, 256), 256, 0, ctx->stream>>>(acc, MV_COPIES, 2 * (int64_t)g, both);
+  SB2_LAUNCH_CHECK(ctx);
+  SB2_CUDA(cudaMemcpyAsync(d_sum, both, sizeof(double) * g, cudaMemcpyDeviceToDevice, ctx->stream));
+  SB2_CUDA(cudaMemcpyAsync(d_sumsq, both + g, sizeof(double) * g, cudaMemcpyDeviceToDevice, ctx->stream));
+  return SB2_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -224,27 +240,16 @@ int32_t sb2_csr_col_sums_f32(sb2_ctx* ctx, int64_t nnz, int32_t g, const int32_t
   SB2_CUDA(cudaSetDevice(ctx->device));
   ScratchScope scr(ctx);
   double *acc, *both;
-  SB2_TRY(scr.alloc(&acc, (size_t)MV_COPIES * 2 * g));
-  SB2_TRY(scr.alloc(&both, (size_t)2 * g));
-  SB2_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * MV_COPIES * 2 * g, ctx->stream));
+  SB2_TRY(alloc_col_stats(ctx, scr, g, &acc, &both));
   if (nnz > 0) {
-    col_sums_transformed_kernel<<<ctx->prop.multiProcessorCount * 8, 256, 0, ctx->stream>>>(nnz, d_indices, d_data, g, apply_expm1,
-                                                                                          (float)log_scale, acc);
+    const unsigned grid = ctx->prop.multiProcessorCount * 8;
+    if (apply_expm1)
+      col_sums_transformed_kernel<true><<<grid, 256, 0, ctx->stream>>>(nnz, d_indices, d_data, g, acc, (float)log_scale);
+    else
+      col_sums_transformed_kernel<false><<<grid, 256, 0, ctx->stream>>>(nnz, d_indices, d_data, g, acc, (float)log_scale);
     SB2_LAUNCH_CHECK(ctx);
   }
-  reduce_copies_kernel<<<(unsigned)ceil_div64(2 * g, 256), 256, 0, ctx->stream>>>(acc, MV_COPIES, 2 * (int64_t)g, both);
-  SB2_LAUNCH_CHECK(ctx);
-  SB2_CUDA(cudaMemcpyAsync(d_sum, both, sizeof(double) * g, cudaMemcpyDeviceToDevice, ctx->stream));
-  SB2_CUDA(cudaMemcpyAsync(d_sumsq, both + g, sizeof(double) * g, cudaMemcpyDeviceToDevice, ctx->stream));
-  return SB2_OK;
-}
-
-static int32_t finish_col_stats(sb2_ctx* ctx, const double* acc, double* both, int32_t g, double* d_sum, double* d_sumsq) {
-  reduce_copies_kernel<<<(unsigned)ceil_div64(2 * g, 256), 256, 0, ctx->stream>>>(acc, MV_COPIES, 2 * (int64_t)g, both);
-  SB2_LAUNCH_CHECK(ctx);
-  SB2_CUDA(cudaMemcpyAsync(d_sum, both, sizeof(double) * g, cudaMemcpyDeviceToDevice, ctx->stream));
-  SB2_CUDA(cudaMemcpyAsync(d_sumsq, both + g, sizeof(double) * g, cudaMemcpyDeviceToDevice, ctx->stream));
-  return SB2_OK;
+  return finish_col_stats(ctx, acc, both, g, d_sum, d_sumsq);
 }
 
 int32_t sb2_csr_col_stats_rows_f32(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_indptr, const int32_t* d_indices,
@@ -253,9 +258,7 @@ int32_t sb2_csr_col_stats_rows_f32(sb2_ctx* ctx, int64_t n, int32_t g, const int
   SB2_CUDA(cudaSetDevice(ctx->device));
   ScratchScope scr(ctx);
   double *acc, *both;
-  SB2_TRY(scr.alloc(&acc, (size_t)MV_COPIES * 2 * g));
-  SB2_TRY(scr.alloc(&both, (size_t)2 * g));
-  SB2_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * MV_COPIES * 2 * g, ctx->stream));
+  SB2_TRY(alloc_col_stats(ctx, scr, g, &acc, &both));
   if (n > 0) {
     col_stats_rows_kernel<<<gridw(n), 256, 0, ctx->stream>>>(n, d_indptr, d_indices, d_data, d_mask, g, acc);
     SB2_LAUNCH_CHECK(ctx);
@@ -292,9 +295,7 @@ int32_t sb2_dense_col_stats(sb2_ctx* ctx, int64_t n, int32_t g, const void* d_x,
   SB2_CUDA(cudaSetDevice(ctx->device));
   ScratchScope scr(ctx);
   double *acc, *both;
-  SB2_TRY(scr.alloc(&acc, (size_t)MV_COPIES * 2 * g));
-  SB2_TRY(scr.alloc(&both, (size_t)2 * g));
-  SB2_CUDA(cudaMemsetAsync(acc, 0, sizeof(double) * MV_COPIES * 2 * g, ctx->stream));
+  SB2_TRY(alloc_col_stats(ctx, scr, g, &acc, &both));
   if (n > 0) {
     const unsigned grid = (unsigned)ceil_div64(n, DS_ROWS);
     if (is_f64) dense_col_stats_kernel<double><<<grid, 256, 0, ctx->stream>>>(n, g, (const double*)d_x, d_mask, acc);

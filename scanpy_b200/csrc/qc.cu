@@ -85,21 +85,6 @@ __device__ void top_sums(const uint32_t* s, int k, int64_t nz, int64_t q, int m,
   __syncthreads();
 }
 
-// sum over the CTA of one value per thread, in a fixed order (warp tree, then warps in order); result on thread 0
-template <typename T>
-__device__ __forceinline__ T block_sum(T v, T* red) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  const int w = threadIdx.x >> 5;
-  if ((threadIdx.x & 31) == 0) red[w] = v;
-  __syncthreads();
-  T s = 0;
-  if (threadIdx.x == 0)
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += red[i];
-  __syncthreads();
-  return s;
-}
-
 struct RowStats {
   int64_t nz, pos;
 };

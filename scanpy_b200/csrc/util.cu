@@ -1,4 +1,7 @@
-// util.cu — small device utilities shared by the graph kernels (prefix sums).
+// util.cu — small utilities shared across files: the device prefix sum of the graph kernels and the host cyclic
+// Jacobi eigensolver of PCA's Rayleigh-Ritz step and eigsh's restart problem.
+#include <math.h>
+
 #include "common.cuh"
 
 namespace {
@@ -89,4 +92,44 @@ int32_t sb2_scan_i32_to_i64(sb2_ctx* ctx, const int32_t* d_in, int64_t n, int64_
   scan_add_kernel<<<(unsigned)ceil_div64(n + 1, 256), 256, 0, ctx->stream>>>(d_out, n, sums, sums + nb);
   SB2_LAUNCH_CHECK(ctx);
   return SB2_OK;
+}
+
+void jacobi_eigh(std::vector<double>& A, int m, std::vector<double>& w, std::vector<double>& V) {
+  V.assign((size_t)m * m, 0.0);
+  for (int i = 0; i < m; ++i) V[(size_t)i * m + i] = 1.0;
+  for (int sweep = 0; sweep < 60; ++sweep) {
+    double off = 0.0, diag = 0.0;
+    for (int i = 0; i < m; ++i) {
+      diag += A[(size_t)i * m + i] * A[(size_t)i * m + i];
+      for (int j = i + 1; j < m; ++j) off += A[(size_t)i * m + j] * A[(size_t)i * m + j];
+    }
+    if (off <= 1e-30 * (diag + off) || off == 0.0) break;
+    for (int p = 0; p < m - 1; ++p) {
+      for (int q = p + 1; q < m; ++q) {
+        const double apq = A[(size_t)p * m + q];
+        if (fabs(apq) < 1e-300) continue;
+        const double app = A[(size_t)p * m + p], aqq = A[(size_t)q * m + q];
+        const double tau = (aqq - app) / (2.0 * apq);
+        const double t = (tau >= 0.0 ? 1.0 : -1.0) / (fabs(tau) + sqrt(1.0 + tau * tau));
+        const double c = 1.0 / sqrt(1.0 + t * t), s = t * c;
+        for (int k = 0; k < m; ++k) {  // columns p,q
+          const double akp = A[(size_t)k * m + p], akq = A[(size_t)k * m + q];
+          A[(size_t)k * m + p] = c * akp - s * akq;
+          A[(size_t)k * m + q] = s * akp + c * akq;
+        }
+        for (int k = 0; k < m; ++k) {  // rows p,q
+          const double apk = A[(size_t)p * m + k], aqk = A[(size_t)q * m + k];
+          A[(size_t)p * m + k] = c * apk - s * aqk;
+          A[(size_t)q * m + k] = s * apk + c * aqk;
+        }
+        for (int k = 0; k < m; ++k) {
+          const double vkp = V[(size_t)k * m + p], vkq = V[(size_t)k * m + q];
+          V[(size_t)k * m + p] = c * vkp - s * vkq;
+          V[(size_t)k * m + q] = s * vkp + c * vkq;
+        }
+      }
+    }
+  }
+  w.resize(m);
+  for (int i = 0; i < m; ++i) w[i] = A[(size_t)i * m + i];
 }
