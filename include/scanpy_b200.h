@@ -329,6 +329,24 @@ int32_t sb2_combat_adjust(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f64,
                           const double* d_beta, const double* d_sqrt_vp, const double* d_gamma, const double* d_dsq,
                           double* d_out);
 
+/* ---- sc.metrics.morans_i / sc.metrics.gearys_c (src/scanpy/metrics/_morans_i.py, _gearys_c.py; csrc/autocorr.cu) ----
+ * X holds all n cells as rows: dense (d_x, row-major [n x g]) or CSR arrays (d_xindptr over all n rows; sorted column
+ * indices, no duplicates; d_x NULL), float32 (is_f64 = 0) or float64 values.  The graph is a block of `rows` rows, cells
+ * row0 .. row0 + rows - 1, as CSR arrays with fp64 weights (d_gindptr pointing at the block's first row, entry offsets
+ * absolute; column indices in [0, n) in any order; explicit zeros, self-loops, empty rows and negative weights allowed).
+ * The per-gene mean comes from sb2_regress_col_sums; Σx and the constancy flag are not recomputed here.
+ * sb2_autocorr_sums <- the arc loops of _morans_i_vec_w and _gearys_c_vec_w.  With z = x - d_mean[j] for gene j, merges
+ *                      into d_acc fp64 [3 x g] (zeroed before the first call): row 0 A = Σ_i z_i Σ_j w_ij z_j (`inum`),
+ *                      row 1 B = Σ_i Σ_j w_ij (x_i - x_j)² (`total`), row 2 Q = Σ_i z_i², summed over the block's rows i
+ *                      and their stored arcs i -> j, in fp64 on the centred and differenced values.  Blocks must be
+ *                      consecutive, and all but the last a multiple of SB2_AUTOCORR_TILE_ROWS rows: the result then has
+ *                      the same bits as one call over all rows. */
+#define SB2_AUTOCORR_TILE_ROWS 1024
+int32_t sb2_autocorr_sums(sb2_ctx* ctx, int64_t row0, int64_t rows, int32_t g, int32_t is_f64, const void* d_x,
+                          const int64_t* d_xindptr, const int32_t* d_xindices, const void* d_xdata,
+                          const int64_t* d_gindptr, const int32_t* d_gindices, const double* d_gweights,
+                          const double* d_mean, double* d_acc);
+
 
 /* ---- extreme eigenpairs of diag(s) A diag(s), A symmetric fp32 CSR (csrc/eigs.cu: thick-restart Lanczos, fp64) ----
  * Replaces `scipy.sparse.linalg.eigsh(matrix.astype(float64), k=n_comps, which='LM', v0=...)` in

@@ -138,6 +138,8 @@ SIGNATURES = {
     "sb2_combat_adjust": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),
+    "sb2_autocorr_sums": (c_int32, [c_void_p, c_int64, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

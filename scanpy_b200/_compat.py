@@ -152,6 +152,27 @@ def is_anndata_like(obj) -> bool:
     return all(hasattr(obj, a) for a in ("X", "obs", "var", "obsm", "varm", "obsp", "uns"))
 
 
+def get_arr(adata, *, use_raw: bool = False, layer=None, obsm=None, obsp=None):
+    """`_get_arr(adata, use_raw=..., layer=..., obsm=..., obsp=...)` along the cells (src/scanpy/get/get.py:545-570)."""
+    if not isinstance(use_raw, bool):
+        raise TypeError(f"use_raw expected to be bool, was {type(use_raw)}.")
+    picked = [k for k, v in (("use_raw", use_raw), ("layer", layer), ("obsm", obsm), ("obsp", obsp))
+              if v is not None and v is not False]
+    if len(picked) > 1:
+        valid = [f"`{k}`" for k in picked]
+        valid[-1] = f"or {valid[-1]}"
+        raise ValueError(f"Only one of {', '.join(valid)} can be specified.")
+    if use_raw:
+        return adata.raw.X
+    if layer is not None:
+        return adata.layers[layer]
+    if obsm is not None:
+        return adata.obsm[obsm]
+    if obsp is not None:
+        return adata.obsp[obsp]
+    return adata.X
+
+
 def as_csr_f32(x):
     """Input matrix -> scipy CSR with float32 data (float64 is down-cast: the kernels compute in fp32
     storage / fp64 accumulation; dense input is converted)."""

@@ -114,7 +114,8 @@ def csr_to_device(x):
 class DeviceX:
     """X on the device by row blocks, for the entry points that take a dense block or CSR arrays of float32 or float64
     values (regress_out, the Pearson residuals): a CSR uploaded once (sorted indices, no duplicates), or a dense array
-    uploaded one block at a time.  `block(r0, r1)` -> (d_x, d_indptr, d_indices, d_data)."""
+    uploaded one block at a time.  A dense CUDA tensor of the value dtype is used where it is, without copies.
+    `block(r0, r1)` -> (d_x, d_indptr, d_indices, d_data)."""
 
     def __init__(self, x, dtype: np.dtype):
         from scipy import sparse
@@ -135,6 +136,8 @@ class DeviceX:
     def block(self, r0: int, r1: int):
         if self.dense is None:
             return None, self.indptr[r0:], self.indices, self.data
+        if hasattr(self.dense, "data_ptr"):  # a CUDA tensor: already on the device
+            return self.dense[r0:r1], None, None, None
         return _to_device(np.ascontiguousarray(self.dense[r0:r1], dtype=self.dtype)), None, None, None
 
     def gather(self, order: np.ndarray, d_order, k0: int, k1: int):

@@ -28,7 +28,7 @@ from scipy import sparse
 
 from . import _abi, _ops
 from ._abi import check, ptr
-from ._compat import accepts_legacy_random_state, is_anndata_like, log_done, log_start, logger, settings, warn
+from ._compat import accepts_legacy_random_state, get_arr, is_anndata_like, log_done, log_start, logger, settings, warn
 from ._regress import _col_sums
 
 PARTIAL_BYTES = 1 << 28  # device scratch for the residual variance's per-subtile partials
@@ -110,23 +110,11 @@ def _residual_variances(dx: _ops.DeviceX, g: int, rows: np.ndarray, d_rows, d_ce
         return acc[2] / acc[0], acc[3]
 
 
-def _get_counts(adata, *, layer=None, obsm=None):
-    """`_get_arr(adata, layer=..., obsm=...)` (src/scanpy/get/get.py:545-570)."""
-    picked = [k for k, v in (("layer", layer), ("obsm", obsm)) if v is not None]
-    if len(picked) > 1:
-        raise ValueError("Only one of `layer`, or `obsm` can be specified.")
-    if layer is not None:
-        return adata.layers[layer]
-    if obsm is not None:
-        return adata.obsm[obsm]
-    return adata.X
-
-
 # ------------------------------------------------------------------------------------------ highly_variable_genes
 def _highly_variable_pearson_residuals(adata, *, theta, clip, n_top_genes, batch_key, check_values, layer, subset,
                                        inplace):
     """_highly_variable_genes.py:129-287."""
-    x = _get_counts(adata, layer=layer)
+    x = get_arr(adata, layer=layer)
     computed_on = layer if layer else "adata.X"
     vdtype = _check_x(x, "highly_variable_genes")
     if not sparse.issparse(x):
@@ -276,7 +264,7 @@ def normalize_pearson_residuals(adata, *, theta: float = 100, clip: float | None
         if not inplace:
             raise ValueError("`copy=True` cannot be used with `inplace=False`.")
         adata = adata.copy()
-    x = _get_counts(adata, layer=layer, obsm=obsm)
+    x = get_arr(adata, layer=layer, obsm=obsm)
     computed_on = layer or obsm or "adata.X"
     start = log_start(f"computing analytic Pearson residuals on {computed_on}")
     residuals = _pearson_residuals(x, theta, clip, check_values)
@@ -344,7 +332,7 @@ def normalize_pearson_residuals_pca(adata, *, theta: float = 100, clip: float | 
         mask_var = "highly_variable" if "highly_variable" in adata.var else None
     mask_var = _check_mask(adata, mask_var, "var")
     _check_theta_clip(theta, clip)
-    counts = _get_counts(adata, layer=layer)
+    counts = get_arr(adata, layer=layer)
     _check_x(counts, "normalize_pearson_residuals")
     if mask_var is not None:
         counts = counts[:, mask_var]
@@ -376,7 +364,7 @@ def recipe_pearson_residuals(adata, *, theta: float = 100, clip: float | None = 
         raise ValueError("`pp.highly_variable_genes` expects an `AnnData` argument, pass `inplace=False` if you want "
                          "to return a `pd.DataFrame`.")
     _check_theta_clip(theta, clip)
-    _check_x(_get_counts(adata, layer=layer), "highly_variable_genes")
+    _check_x(get_arr(adata, layer=layer), "highly_variable_genes")
     hvg_args = dict(flavor="pearson_residuals", n_top_genes=n_top_genes, batch_key=batch_key, theta=theta, clip=clip,
                     chunksize=chunksize, check_values=check_values, layer=layer)
     if inplace:
@@ -387,7 +375,7 @@ def recipe_pearson_residuals(adata, *, theta: float = 100, clip: float | None = 
         mask = np.asarray(hvg["highly_variable"], dtype=bool)
     adata_pca = adata[:, mask].copy()
     if layer is not None:
-        adata_pca.X = _get_counts(adata, layer=layer)[:, mask].copy()
+        adata_pca.X = get_arr(adata, layer=layer)[:, mask].copy()
     normalize_pearson_residuals(adata_pca, theta=theta, clip=clip, check_values=check_values)
     pca(adata_pca, n_comps=n_comps, rng=rng, **kwargs_pca)
     if inplace:

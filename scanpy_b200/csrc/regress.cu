@@ -99,31 +99,6 @@ col_sums_kernel(int64_t rows, int g, const T* __restrict__ x, const int64_t* __r
   pnan[sub * g + c] = nan;
 }
 
-// acc[i] += part[0][i] + ... in subtile order; the per-gene min / max / NaN likewise
-__global__ void fold_kernel(int64_t nsub, int64_t width, int g, const double* __restrict__ part,
-                            const double* __restrict__ pmin, const double* __restrict__ pmax,
-                            const int32_t* __restrict__ pnan, double* __restrict__ acc, double* __restrict__ cmin,
-                            double* __restrict__ cmax, int32_t* __restrict__ cnan) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < width) {
-    double s = acc[i];
-    for (int64_t t = 0; t < nsub; ++t) s += part[t * width + i];
-    acc[i] = s;
-  }
-  if (i < g) {
-    double a = cmin[i], b = cmax[i];
-    int32_t f = cnan[i];
-    for (int64_t t = 0; t < nsub; ++t) {
-      a = fmin(a, pmin[t * g + i]);
-      b = fmax(b, pmax[t * g + i]);
-      f |= pnan[t * g + i];
-    }
-    cmin[i] = a;
-    cmax[i] = b;
-    cnan[i] = f;
-  }
-}
-
 // grid (row tiles of SLAB_ROWS, slabs)
 template <typename T, typename O, bool CSR, int KMAX>
 __global__ void __launch_bounds__(SLAB_THREADS)
@@ -209,8 +184,8 @@ int32_t sb2_regress_col_sums(sb2_ctx* ctx, int64_t rows, int32_t g, int32_t is_f
   });
   SB2_LAUNCH_CHECK(ctx);
   const int64_t span = width > g ? width : g;
-  fold_kernel<<<(unsigned)ceil_div64(span, 256), 256, 0, ctx->stream>>>(nsub, width, g, part, pmin, pmax, pnan, d_acc,
-                                                                       d_min, d_max, d_nan);
+  fold_kernel<><<<(unsigned)ceil_div64(span, 256), 256, 0, ctx->stream>>>(nsub, width, g, part, pmin, pmax, pnan, d_acc,
+                                                                         d_min, d_max, d_nan);
   SB2_LAUNCH_CHECK(ctx);
   return SB2_OK;
 }

@@ -1,4 +1,4 @@
-// slab.cuh — the column-slab scheme of the dense per-gene passes (regress.cu, pearson.cu, combat.cu).
+// slab.cuh — the column-slab scheme of the dense per-gene passes (regress.cu, pearson.cu, combat.cu, autocorr.cu).
 //
 // One CTA owns a SLAB_THREADS-column slab of a block of rows and each thread one column.  A CSR input is read in place:
 // the CTA binary-searches its slab in each of SLAB_ROWS rows (column indices sorted, no duplicates) and scatters the
@@ -17,7 +17,8 @@ constexpr int SLAB_THREADS = 256;  // one column per thread: 256-column slabs
 constexpr int SLAB_ROWS = 16;      // rows staged per step
 constexpr int SLAB_TILE = 1024;    // rows per subtile
 static_assert(SLAB_TILE == SB2_REGRESS_TILE_ROWS && SLAB_TILE == SB2_PEARSON_TILE_ROWS &&
-              SLAB_TILE == SB2_COMBAT_TILE_ROWS && SLAB_TILE % SLAB_ROWS == 0, "subtile");
+              SLAB_TILE == SB2_COMBAT_TILE_ROWS && SLAB_TILE == SB2_AUTOCORR_TILE_ROWS && SLAB_TILE % SLAB_ROWS == 0,
+              "subtile");
 
 // The slab [c0, c1) of the m rows rid[0..m) of a CSR, scattered into tile[r][col - c0]; tile must be zero on entry.
 // Thread r < m has written rid[r] before the call; the caller clears what it reads.
@@ -46,6 +47,33 @@ __device__ __forceinline__ void stage_csr(const int64_t* __restrict__ indptr, co
   for (int r = warp; r < m; r += SLAB_THREADS / 32)
     for (int64_t e = lo[r] + lane; e < hi[r]; e += 32) tile[r][indices[e] - c0] = data[e];
   __syncthreads();
+}
+
+// acc[i] += part[0][i] + ... in subtile order; the per-gene min / max / NaN likewise (g = 0: sums only, and pmin, pmax,
+// pnan, cmin, cmax, cnan may be NULL).  A template only so that the units that do not launch it do not compile it.
+template <int = 0>
+__global__ void fold_kernel(int64_t nsub, int64_t width, int g, const double* __restrict__ part,
+                            const double* __restrict__ pmin, const double* __restrict__ pmax,
+                            const int32_t* __restrict__ pnan, double* __restrict__ acc, double* __restrict__ cmin,
+                            double* __restrict__ cmax, int32_t* __restrict__ cnan) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < width) {
+    double s = acc[i];
+    for (int64_t t = 0; t < nsub; ++t) s += part[t * width + i];
+    acc[i] = s;
+  }
+  if (i < g) {
+    double a = cmin[i], b = cmax[i];
+    int32_t f = cnan[i];
+    for (int64_t t = 0; t < nsub; ++t) {
+      a = fmin(a, pmin[t * g + i]);
+      b = fmax(b, pmax[t * g + i]);
+      f |= pnan[t * g + i];
+    }
+    cmin[i] = a;
+    cmax[i] = b;
+    cnan[i] = f;
+  }
 }
 
 // acc[k][j] (k = 0 count, 1 mean, 2 M2, and with SUM_SQ 3 Σx²) merged with the SLAB_TILE-row subtiles' partials
