@@ -353,7 +353,10 @@ int32_t sb2_autocorr_sums(sb2_ctx* ctx, int64_t row0, int64_t rows, int32_t g, i
  * Neighbors.compute_eigen (src/scanpy/neighbors/__init__.py:832-884; sc.tl.diffmap) and the eigsh of umap's spectral
  * initialisation (sc.tl.umap).  d_scale may be NULL (s = 1).  which: 0 largest algebraic, 1 largest magnitude, 2 smallest
  * algebraic.  ncv <= 0 / tol <= 0 / max_restarts <= 0 pick defaults (max(2 nev + 16, 40), 1e-10, 400).  h_evals ascending
- * like eigsh; d_evecs fp64 [nev x n], row e = unit eigenvector of h_evals[e] (sign arbitrary, as with ARPACK). */
+ * like eigsh; d_evecs fp64 [nev x n], row e = unit eigenvector of h_evals[e] (sign arbitrary, as with ARPACK).
+ * A converged set is locked and searched again from a fresh start vector for copies of its eigenvalues that the start
+ * vector missed.  info: n_converged = returned pairs whose residual estimate |beta_m y_m| is <= tol * max|theta|;
+ * max_residual = the largest such estimate over the returned pairs, taken in the cycle that locked each pair. */
 typedef struct sb2_eigs_info {
   int32_t restarts, matvecs, n_converged, reserved;
   double max_residual;

@@ -127,3 +127,10 @@ __device__ __forceinline__ T block_sum(T v, T* red) {
 int32_t sb2_scan_i32_to_i64(sb2_ctx* ctx, const int32_t* d_in, int64_t n, int64_t* d_out);
 // host cyclic Jacobi: A (m x m symmetric, row-major, destroyed) -> eigenvalues w, eigenvectors V (columns)
 void jacobi_eigh(std::vector<double>& A, int m, std::vector<double>& w, std::vector<double>& V);
+
+// ---- eigs.cu ----
+// sb2_eigsh_csr_scaled with the search for missed copies of the wanted eigenvalues made optional: without it, the first
+// set whose residuals converge is returned (the UMAP spectral initialisation, which lays out a disconnected graph as one)
+int32_t eigsh_csr_scaled(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, const int32_t* d_indices, const float* d_weights,
+                         const double* d_scale, int32_t nev, int32_t which, int32_t ncv, double tol, int32_t max_restarts,
+                         const double* d_v0, double* h_evals, double* d_evecs, sb2_eigs_info* info, bool lock_and_search);

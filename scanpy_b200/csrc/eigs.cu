@@ -87,6 +87,15 @@ __global__ void eig_scale_kernel(int64_t n, const double* __restrict__ w, const 
   const double nr = sqrt(*nrm2);
   out[i] = nr > 0.0 ? w[i] / nr : 0.0;
 }
+// out[i] = splitmix64(i, salt) mapped to [-1, 1): a start vector unrelated to any Krylov space met so far
+__global__ void eig_fresh_kernel(int64_t n, uint64_t salt, double* __restrict__ out) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  uint64_t z = (uint64_t)i + 0x9E3779B97F4A7C15ull * salt;
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  out[i] = (double)((z ^ (z >> 31)) >> 11) * (2.0 / 9007199254740992.0) - 1.0;
+}
 // Vout[:, j0 + t] = V[:, :m] Y[:, t], t < nt <= 8  (Y column-major m x nt in shared memory)
 __global__ void __launch_bounds__(256)
 eig_rotate_kernel(int64_t n, int m, int nt, const double* __restrict__ V, int64_t ld, const double* __restrict__ Y,
@@ -168,6 +177,13 @@ extern "C" int32_t sb2_eigsh_csr_scaled(sb2_ctx* ctx, int64_t n, const int64_t* 
                                         const float* d_weights, const double* d_scale, int32_t nev, int32_t which,
                                         int32_t ncv, double tol, int32_t max_restarts, const double* d_v0,
                                         double* h_evals, double* d_evecs, sb2_eigs_info* info) {
+  return eigsh_csr_scaled(ctx, n, d_indptr, d_indices, d_weights, d_scale, nev, which, ncv, tol, max_restarts, d_v0, h_evals,
+                          d_evecs, info, true);
+}
+
+int32_t eigsh_csr_scaled(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, const int32_t* d_indices, const float* d_weights,
+                         const double* d_scale, int32_t nev, int32_t which, int32_t ncv, double tol, int32_t max_restarts,
+                         const double* d_v0, double* h_evals, double* d_evecs, sb2_eigs_info* info, bool lock_and_search) {
   SB2_CHECK_ARG(ctx && d_indptr && d_indices && d_weights && d_v0 && h_evals && d_evecs, "null pointer");
   SB2_CHECK_ARG(n >= 2 && n < INT32_MAX, "n");
   SB2_CHECK_ARG(nev >= 1 && nev < n && nev <= 64, "nev must be in [1, min(n-1, 64)]");
@@ -198,7 +214,14 @@ extern "C" int32_t sb2_eigsh_csr_scaled(sb2_ctx* ctx, int64_t n, const int64_t* 
 
   std::vector<double> T((size_t)m * m, 0.0), Tw, theta, Y, hh(2 * (m + 2));
   std::vector<int> order(m);
-  int k = 0, restarts = 0, n_conv = 0, matvecs = 0;
+  // locked[p]: basis vector p is a converged Ritz vector of an earlier cycle, kept with no coupling to the rest.  A single
+  // start vector meets a repeated eigenvalue in one direction only (more copies appear only through rounding), so a set
+  // that has converged is locked and searched again from a fresh start vector orthogonal to it; it is final once the
+  // best Ritz value of that search has converged without displacing any of the set.  lres[p]: the residual estimate of
+  // locked vector p in the cycle that locked it (its estimate in later cycles is exactly 0: it has no coupling).
+  std::vector<char> locked(m + 1, 0), locked_next(m + 1, 0);
+  std::vector<double> lres(m + 1, 0.0), lres_next(m + 1, 0.0);
+  int k = 0, restarts = 0, n_conv = 0, matvecs = 0, nlock = 0;
   for (;;) {
     int me = m;           // effective basis size of this cycle (< m only on an exact invariant subspace)
     double beta_m = 0.0;  // coupling of the residual vector V_me
@@ -238,18 +261,54 @@ extern "C" int32_t sb2_eigsh_csr_scaled(sb2_ctx* ctx, int64_t n, const int64_t* 
     std::iota(order.begin(), order.end(), 0);
     auto key = [&](int i) { return which == 1 ? fabs(theta[i]) : which == 0 ? theta[i] : -theta[i]; };
     std::sort(order.begin(), order.end(), [&](int a, int b) { return key(a) > key(b); });
+    // Ritz vector i lies in the locked block iff its components outside it are zero (T is block diagonal there); it is
+    // then locked vector lock_pos(i) itself (the diagonal block is never rotated)
+    auto in_lock = [&](int i) {
+      if (nlock == 0) return false;
+      for (int r = 0; r < me; ++r)
+        if (!locked[r] && Y[(size_t)r * me + i] != 0.0) return false;
+      return true;
+    };
+    auto lock_pos = [&](int i) {
+      int p = 0;
+      for (int r = 0; r < me; ++r)
+        if (Y[(size_t)r * me + i] != 0.0) p = r;
+      return p;
+    };
+    auto res_of = [&](int i) { return in_lock(i) ? lres[lock_pos(i)] : fabs(beta_m * Y[(size_t)(me - 1) * me + i]); };
     n_conv = 0;
     double tnorm = 0.0;
     for (int i = 0; i < me; ++i) tnorm = std::max(tnorm, fabs(theta[i]));
-    double max_res = 0.0;
-    for (int e = 0; e < nev; ++e) {
-      const double res = fabs(beta_m * Y[(size_t)(me - 1) * me + order[e]]);
-      max_res = std::max(max_res, res);
-      if (res <= tol * std::max(tnorm, 1e-300)) ++n_conv;
+    for (int e = 0; e < nev; ++e)
+      if (res_of(order[e]) <= tol * std::max(tnorm, 1e-300)) ++n_conv;
+    bool verified = false, relock = false;
+    if (n_conv == nev && !lock_and_search) {
+      verified = true;
+    } else if (n_conv == nev) {
+      if (nlock == 0) {
+        relock = true;
+      } else {
+        double kmin = INFINITY;
+        int best = -1;
+        for (int i = 0; i < me; ++i) {
+          if (in_lock(i)) kmin = std::min(kmin, key(i));
+          else if (best < 0 || key(i) > key(best)) best = i;
+        }
+        if (best < 0 || res_of(best) <= tol * std::max(tnorm, 1e-300)) {
+          if (best < 0 || key(best) <= kmin + 1e-12 * tnorm) verified = true;
+          else relock = true;  // a new Ritz value displaces the locked set: lock the new wanted set and search again
+        }
+      }
     }
-    const bool done = n_conv == nev || restarts >= max_restarts || beta_m == 0.0;
-    // Ritz vectors to keep: the wanted nev (final) or nev + a share of the rest (thick restart)
-    const int kk = done ? nev : std::min(me - 1, nev + std::max(2, (me - nev) / 2));
+    if (verified && nlock > 0)  // the locked Ritz vectors are the result, ahead of any tie from the last search
+      std::stable_partition(order.begin(), order.end(), [&](int i) { return in_lock(i); });
+    const bool done = verified || restarts >= max_restarts;
+    // Ritz vectors to keep: the wanted nev (final or locked) or nev + a share of the rest (thick restart)
+    const int kk = done || relock ? nev : std::min(me - 1, nev + std::max(2, (me - nev) / 2));
+    for (int i = 0; i < kk; ++i) {
+      locked_next[i] = relock || in_lock(order[i]);
+      lres_next[i] = res_of(order[i]);
+    }
     std::vector<double> Ycols((size_t)m * 8);
     for (int j0 = 0; j0 < kk; j0 += 8) {
       const int nt = std::min(8, kk - j0);
@@ -272,6 +331,8 @@ extern "C" int32_t sb2_eigsh_csr_scaled(sb2_ctx* ctx, int64_t n, const int64_t* 
       }
       SB2_CUDA(cudaStreamSynchronize(st));
       if (info) {
+        double max_res = 0.0;
+        for (int e = 0; e < nev; ++e) max_res = std::max(max_res, res_of(order[e]));
         info->restarts = restarts;
         info->matvecs = matvecs;
         info->n_converged = n_conv;
@@ -279,14 +340,33 @@ extern "C" int32_t sb2_eigsh_csr_scaled(sb2_ctx* ctx, int64_t n, const int64_t* 
       }
       return SB2_OK;
     }
-    // thick restart: V <- [kept Ritz vectors, residual vector], T <- arrowhead
-    SB2_CUDA(cudaMemcpyAsync(V2 + (size_t)kk * n, V + (size_t)m * n, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
-    std::swap(V, V2);
     std::fill(T.begin(), T.end(), 0.0);
-    for (int i = 0; i < kk; ++i) {
-      T[(size_t)i * m + i] = theta[order[i]];
-      const double c = beta_m * Y[(size_t)(me - 1) * me + order[i]];
-      T[(size_t)i * m + kk] = T[(size_t)kk * m + i] = c;
+    std::fill(locked.begin(), locked.end(), 0);
+    std::copy(locked_next.begin(), locked_next.begin() + kk, locked.begin());
+    std::copy(lres_next.begin(), lres_next.begin() + kk, lres.begin());
+    nlock = (int)std::count(locked.begin(), locked.end(), 1);
+    if (relock) {
+      // V <- [wanted Ritz vectors (locked), fresh start vector orthogonal to them], T <- diagonal
+      eig_fresh_kernel<<<gn, 256, 0, st>>>(n, (uint64_t)(restarts + 1), wv);
+      SB2_LAUNCH_CHECK(ctx);
+      std::swap(V, V2);
+      for (int pass = 0; pass < 2; ++pass) {
+        SB2_TRY(E.dots(kk, V, wv, E.h));
+        SB2_TRY(E.axpy(kk, V, E.h, wv));
+      }
+      SB2_TRY(E.dots(1, wv, wv, E.h + 2 * (m + 2) - 1));
+      eig_scale_kernel<<<gn, 256, 0, st>>>(n, wv, E.h + 2 * (m + 2) - 1, V + (size_t)kk * n);
+      SB2_LAUNCH_CHECK(ctx);
+      for (int i = 0; i < kk; ++i) T[(size_t)i * m + i] = theta[order[i]];
+    } else {
+      // thick restart: V <- [kept Ritz vectors, residual vector], T <- arrowhead (locked rows have no coupling)
+      SB2_CUDA(cudaMemcpyAsync(V2 + (size_t)kk * n, V + (size_t)m * n, sizeof(double) * n, cudaMemcpyDeviceToDevice, st));
+      std::swap(V, V2);
+      for (int i = 0; i < kk; ++i) {
+        T[(size_t)i * m + i] = theta[order[i]];
+        const double c = beta_m * Y[(size_t)(me - 1) * me + order[i]];
+        T[(size_t)i * m + kk] = T[(size_t)kk * m + i] = c;
+      }
     }
     k = kk;
     ++restarts;

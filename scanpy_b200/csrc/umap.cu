@@ -80,11 +80,12 @@ umap_epoch_kernel(int32_t n, const int64_t* __restrict__ indptr, const int32_t* 
         for (int d = 0; d < DIM; ++d) cur[d] += clip4(gc * (cur[d] - oth[d])) * alpha;
       }
     }
-    // negative samples owed since the previous sample of this edge (umap's epoch_of_next_negative_sample bookkeeping)
-    const double rate_e = (double)neg_rate / epd;  // 1 / epochs_per_negative_sample
-    const int64_t c_now = (int64_t)floor(nd * rate_e);
+    // negative samples owed since the previous sample of this edge (umap's epoch_of_next_negative_sample bookkeeping):
+    // floor(epoch * rate / eps) with the integer product divided last, so that it is exact when eps divides it
+    const double rate = (double)neg_rate;
+    const int64_t c_now = (int64_t)floor(nd * rate / epd);
     int64_t c_prev = 1;
-    if (cnt > 1) c_prev = (int64_t)floor(ceil((double)(cnt - 1) * epd) * rate_e);
+    if (cnt > 1) c_prev = (int64_t)floor(ceil((double)(cnt - 1) * epd) * rate / epd);
     if (c_prev < 1) c_prev = 1;
     const int n_neg = (int)min((int64_t)64, max((int64_t)0, c_now - c_prev));
     uint32_t h = hash32(seed ^ hash32((uint32_t)epoch * 0x9E3779B9U + (uint32_t)(e & 0xffffffffu)));
@@ -210,9 +211,10 @@ int32_t sb2_umap_spectral_init_f32(sb2_ctx* ctx, int64_t n, const int64_t* d_ind
   SB2_LAUNCH_CHECK(ctx);
   double evals[17];
   sb2_eigs_info inf{};
-  // umap: eigsh(L, k+1, which='SM', ncv=max(2k+1, sqrt(n)), tol=1e-4); an initialisation does not need more
-  int32_t rc = sb2_eigsh_csr_scaled(ctx, n, d_indptr, d_indices, d_weights, s, nev, 0, std::max(2 * nev + 16, 40), 1e-5, 60, v0,
-                                    evals, evecs, &inf);
+  // umap: eigsh(L, k+1, which='SM', ncv=max(2k+1, sqrt(n)), tol=1e-4); an initialisation does not need more.  No search
+  // for missed copies of eigenvalue 1: on a disconnected graph they would collapse each component to a point
+  int32_t rc = eigsh_csr_scaled(ctx, n, d_indptr, d_indices, d_weights, s, nev, 0, std::max(2 * nev + 16, 40), 1e-5, 60, v0,
+                                evals, evecs, &inf, false);
   if (rc != SB2_OK) return rc;
   const unsigned ge = (unsigned)ceil_div64(n * dim, 256);
   umap_spectral_pick_kernel<<<ge, 256, 0, st>>>(n, dim, nev, evecs, d_init);
