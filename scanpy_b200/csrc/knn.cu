@@ -25,6 +25,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "knn_internal.cuh"
 
@@ -507,22 +509,91 @@ struct EventPairs {  // CUDA-event brackets around the sweep kernels of one call
   }
 };
 
-int32_t launch_rescore(sb2_ctx* ctx, int list_m, int sub, const float* d_x, int64_t n_points, int d, int64_t q0, int64_t ql_base,
-                       const int32_t* row_map, int64_t n_rows, int k, const float* cand_score, const int32_t* cand_idx,
-                       const unsigned int* maxnorm, const float* inv_s2, double c_q, double c_n, const float* dnorm,
-                       const unsigned int* dmax_bits, int32_t* d_idx,
-                       double* d_dist, int32_t* wq, double* wub, unsigned long long* wcnt) {
+// Every run-time switch of the kNN, parsed on every call (the tests change them between calls)
+KnnSwitches knn_switches() {
+  const auto is = [](const char* name, const char* value) {
+    const char* e = getenv(name);
+    return e && strcmp(e, value) == 0;
+  };
+  KnnSwitches s;
+  s.ffma = is("SB2_KNN_PASS1", "ffma");
+  s.split_only = is("SB2_KNN_TIERS", "3");
+  s.big_list = is("SB2_KNN_LIST", "64") || is("SB2_KNN_LIST", "128");
+  if (const char* e = getenv("SB2_KNN_EST")) {
+    if (atoi(e) > 0) s.est_stride = atoi(e);
+    else s.cold = true;
+  }
+  if (const char* e = getenv("SB2_KNN_EST_RANK"); e && atoi(e) >= 1 && atoi(e) <= EST_R) s.est_rank = atoi(e);
+  if (const char* e = getenv("SB2_KNN_SCAN_SLOTS")) s.scan_slots = atoll(e);  // 0 forces the re-sweep (tests)
+  s.pipe = !is("SB2_KNN_PIPE", "0");
+  s.stamps = is("SB2_KNN_STAMPS", "1");
+  s.int_scan = !is("SB2_KNN_SCAN", "float");
+  return s;
+}
+
+// Xt: the points in tiles of 128, k-major, with the row of -|x|^2/2; maxnorm[4]: [0] the bits of the largest squared
+// norm, the rest zeroed for the fp16 tier
+int32_t prep_points(sb2_ctx* ctx, ScratchScope& scr, const float* d_x, int64_t n_points, int d, float** Xt,
+                    unsigned int** maxnorm) {
+  const int64_t n_tiles = ceil_div64(n_points, TILE);
+  SB2_TRY(scr.alloc(Xt, (size_t)(n_tiles * (d + 1) * TILE)));
+  SB2_TRY(scr.alloc(maxnorm, 4));
+  SB2_CUDA(cudaMemsetAsync(*maxnorm, 0, 16, ctx->stream));
+  const size_t smem = (size_t)TILE * d * sizeof(float);
+  SB2_CUDA(cudaFuncSetAttribute(knn_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  knn_prep_kernel<<<(unsigned)n_tiles, 256, smem, ctx->stream>>>(d_x, n_points, d, *Xt, *maxnorm);
+  SB2_LAUNCH_CHECK(ctx);
+  return SB2_OK;
+}
+
+// what the passes of one sb2_knn_l2_f32 call share
+struct KnnCall {
+  sb2_ctx* ctx;
+  ScratchScope* scr;
+  KnnSwitches sw;
+  const float* d_x;
+  int64_t n_points, q0, n_query;
+  int d, k;
+  int32_t* d_idx;
+  double* d_dist;
+  float* Xt = nullptr;
+  unsigned int* maxnorm = nullptr;   // bits of [0] the largest squared norm, [1] the fp16 tier's largest |x - fp16(x)|
+  int32_t* wq[2] = {};               // local rows left open: [0] by tier 1, [1] for the exact scan
+  double* wub[2] = {};               // their bounds on the k-th squared distance
+  unsigned long long* wcnt = nullptr;  // [2] the two queues' lengths
+  int list_m = 0, sub = 0;           // proposals per row, in sub-lists of sub
+  float* cand_score = nullptr;       // [n_query][list_m]
+  int32_t* cand_idx = nullptr;
+  double issued_flops = 0.0;
+  int64_t n_resweep = 0;
+  EventPairs evs;
+};
+
+// how a pass's proposals are certified: |s_computed - s_true| <= c_q |q| R + c_n R^2 / 2 (scores in units of inv_s2 on
+// the tensor path), plus the measured |x - fp16(x)| term of the fp16 tier; the rows it cannot certify join queue `queue`
+struct Bound {
+  double c_q, c_n;
+  const float* inv_s2;
+  const float* dnorm;
+  const unsigned int* dmax;
+  int queue;
+};
+
+// fp64 re-score + certificate of n_rows proposal lists: launch row i is local row ql0 + i, or row_map[i] (ql0 = 0)
+int32_t launch_rescore(KnnCall& c, const Bound& b, int64_t ql0, const int32_t* row_map, int64_t n_rows) {
   if (n_rows == 0) return SB2_OK;
   const int wpb = 8;
   const unsigned grid = (unsigned)ceil_div64(n_rows, wpb);
-#define SB2_RESCORE(RR)                                                                                                          \
-  knn_rescore_kernel<RR><<<grid, wpb * 32, 0, ctx->stream>>>(d_x, n_points, d, q0, ql_base, row_map, n_rows, k, sub, cand_score, \
-                                                             cand_idx, maxnorm, inv_s2, c_q, c_n, dnorm, dmax_bits, d_idx, d_dist, wq, wub, wcnt)
-  if (list_m == 32) SB2_RESCORE(1);
-  else if (list_m == 64) SB2_RESCORE(2);
-  else SB2_RESCORE(4);
-#undef SB2_RESCORE
-  SB2_LAUNCH_CHECK(ctx);
+  const auto launch = [&](auto r) {
+    knn_rescore_kernel<r><<<grid, wpb * 32, 0, c.ctx->stream>>>(
+        c.d_x, c.n_points, c.d, c.q0, ql0, row_map, n_rows, c.k, c.sub, c.cand_score + ql0 * c.list_m,
+        c.cand_idx + ql0 * c.list_m, c.maxnorm, b.inv_s2, b.c_q, b.c_n, b.dnorm, b.dmax, c.d_idx, c.d_dist, c.wq[b.queue],
+        c.wub[b.queue], c.wcnt + b.queue);
+  };
+  if (c.list_m == 32) launch(std::integral_constant<int, 1>());
+  else if (c.list_m == 64) launch(std::integral_constant<int, 2>());
+  else launch(std::integral_constant<int, 4>());
+  SB2_LAUNCH_CHECK(c.ctx);
   return SB2_OK;
 }
 
@@ -534,42 +605,22 @@ int32_t read_count(sb2_ctx* ctx, const unsigned long long* d_cnt, int64_t* out) 
   return SB2_OK;
 }
 
-// ---- the tensor-core sweep of knn_tc2.cu behind the interface tensor_tiers uses ----
-struct SweepV2 {   // knn_tc2.cu: 128-query CTAs x 128-candidate tiles (wgmma N = 128), four sub-lists per row
+// one precision tier of the tensor path (knn_tc2.cu): its sweep shape, its candidate image and its certificate
+struct Tier {
   KnnTc2Shape sh;
-  bool shape(const sb2_ctx* ctx, int d, int terms) { return knn_tc2_shape(ctx, d, terms, terms == 1, &sh); }
-  static int list_m(int k, bool force_big) { return (k > 24 || force_big) ? 128 : 64; }
-  static int sub(int list_m) { return list_m / 4; }
-  int wave_rows(const sb2_ctx* ctx) const { return ctx->prop.multiProcessorCount * TILE; }
-  size_t a_halves(int64_t n) const { return knn_tc2_a_halves(sh, n); }
-  size_t b_halves(int64_t n) const { return knn_tc2_b_halves(sh, n); }
-  int32_t build(sb2_ctx* ctx, const float* x, int64_t n, int d, const unsigned int* mn, const int32_t* g, int64_t gb, __half* A,
-                __half* B, float* inv_s2, float* dnorm, unsigned int* dmax) const {
-    return knn_tc2_build_images(ctx, sh, x, n, d, mn, g, gb, A, B, inv_s2, dnorm, dmax);
-  }
-  int32_t sweep(sb2_ctx* ctx, const __half* A, int64_t a_tile0, const __half* B, int64_t n_points, int64_t n_query, int lm,
-                float* cs, int32_t* ci, double* fl, bool est) const {
-    return knn_tc2_sweep(ctx, sh, A, a_tile0, B, n_points, n_query, lm, cs, ci, fl, est);
-  }
-  void coefs(double* cq, double* cn) const { knn_tc2_error_coefs(sh, cq, cn); }
+  __half* B = nullptr;
+  Bound bound;
 };
 
-struct TierState {
-  sb2_ctx* ctx;
-  ScratchScope* scr;
-  const float* d_x;
-  int64_t n_points, q0, n_query;
-  int d, k;
-  unsigned int* maxnorm;
-  int32_t *wq1, *wq2;
-  double *wub1, *wub2;
-  unsigned long long* wcnt;
-  int32_t* d_idx;
-  double* d_dist;
-  EventPairs* evs;
-  double issued_flops = 0.0;
-  int64_t n_resweep = 0;
-};
+// one sweep of a tier, bracketed by the call's events, and the re-score of its proposals: local rows [ql0, ql0 + n_rows)
+// of the query image A, or (ql0 = 0) the rows row_map[0, n_rows) that A holds gathered in that order
+int32_t sweep_and_certify(KnnCall& c, const Tier& t, const __half* A, int64_t ql0, const int32_t* row_map, int64_t n_rows) {
+  SB2_TRY(c.evs.begin());
+  SB2_TRY(knn_tc2_sweep(c.ctx, c.sw, t.sh, A, row_map ? 0 : (c.q0 + ql0) / TILE, t.B, c.n_points, n_rows, c.list_m,
+                        c.cand_score + ql0 * c.list_m, c.cand_idx + ql0 * c.list_m, &c.issued_flops));
+  SB2_TRY(c.evs.end());
+  return launch_rescore(c, t.bound, ql0, row_map, n_rows);
+}
 
 // Tensor path, in tiers that each end in the same fp64 re-score + certificate:
 //   tier 1  one fp16 sweep (K = d+3): proposals whose rounding bound (2^-10 |q| R) still certifies the exact top-k are final
@@ -577,103 +628,109 @@ struct TierState {
 //   tier 3  rows still open (exact ties at the k-th distance, floods of duplicates): fp64 scan of every point (caller)
 // A pilot of one wave of CTAs measures tier 1's certification rate; if most rows fail (data far from the origin,
 // tiny neighbour gaps) the remaining rows go straight to the split-precision sweep.
-template <class SW>
-int32_t tensor_tiers(TierState& t, bool split_only, bool force_big_list) {
-  sb2_ctx* ctx = t.ctx;
-  ScratchScope& scr = *t.scr;
-  cudaStream_t st = ctx->stream;
-  const int64_t n_points = t.n_points, n_query = t.n_query, q0 = t.q0;
-  const int d = t.d, k = t.k;
-  SW s1, s3;
-  SB2_CHECK_ARG(s1.shape(ctx, d, 1) && s3.shape(ctx, d, 3), "tensor-core kNN tile does not fit shared memory");
-  const int list_m = SW::list_m(k, force_big_list), sub = SW::sub(list_m);
-  float* cand_score;
-  int32_t* cand_idx;
-  SB2_TRY(scr.alloc(&cand_score, (size_t)n_query * list_m));
-  SB2_TRY(scr.alloc(&cand_idx, (size_t)n_query * list_m));
+int32_t tensor_tiers(KnnCall& c) {
+  sb2_ctx* ctx = c.ctx;
+  ScratchScope& scr = *c.scr;
+  const int64_t n_points = c.n_points, n_query = c.n_query;
+  const int d = c.d;
+  // only tier 1 starts from a sampled threshold: a row the re-sweep gathers may have failed because its sampled
+  // threshold was too tight (fewer than k candidates beat it), and must not fail twice
+  Tier t1, t3;
+  SB2_CHECK_ARG(knn_tc2_shape(ctx, d, 1, true, &t1.sh) && knn_tc2_shape(ctx, d, 3, false, &t3.sh),
+                "tensor-core kNN tile does not fit shared memory");
+  c.list_m = (c.k > 24 || c.sw.big_list) ? 128 : 64;
+  c.sub = c.list_m / 4;  // four sub-lists per row
+  SB2_TRY(scr.alloc(&c.cand_score, (size_t)n_query * c.list_m));
+  SB2_TRY(scr.alloc(&c.cand_idx, (size_t)n_query * c.list_m));
   float* inv_s2;
   SB2_TRY(scr.alloc(&inv_s2, 4));
-  double cq1, cn1, cq3, cn3;
-  s1.coefs(&cq1, &cn1);
-  s3.coefs(&cq3, &cn3);
-  __half *A1 = nullptr, *B1 = nullptr, *A3 = nullptr, *B3 = nullptr;
-  float* dnorm = nullptr;  // |x - fp16(x)| per point; its maximum lives in maxnorm[1]
-  unsigned int* maxnorm = t.maxnorm;
-  const int64_t qt0 = q0 / TILE;
+  t1.bound = {0.0, 0.0, inv_s2, nullptr, nullptr, 0};  // tier 1's open rows wait for the re-sweep,
+  t3.bound = {0.0, 0.0, inv_s2, nullptr, nullptr, 1};  // the split tier's for the exact scan
+  knn_tc2_error_coefs(t1.sh, &t1.bound.c_q, &t1.bound.c_n);
+  knn_tc2_error_coefs(t3.sh, &t3.bound.c_q, &t3.bound.c_n);
   int64_t done = 0;  // local rows [0, done) have been through their first sweep
-  bool direct_split = split_only;
-  if (!split_only) {
-    SB2_TRY(scr.alloc(&A1, s1.a_halves(n_points)));
-    SB2_TRY(scr.alloc(&B1, s1.b_halves(n_points)));
+  if (!c.sw.split_only) {
+    __half* A1;
+    float* dnorm;  // |x - fp16(x)| per point; its maximum lives in maxnorm[1]
+    SB2_TRY(scr.alloc(&A1, knn_tc2_a_halves(t1.sh, n_points)));
+    SB2_TRY(scr.alloc(&t1.B, knn_tc2_b_halves(t1.sh, n_points)));
     SB2_TRY(scr.alloc(&dnorm, (size_t)n_points));
-    SB2_TRY(s1.build(ctx, t.d_x, n_points, d, maxnorm, nullptr, 0, A1, B1, inv_s2, dnorm, maxnorm + 1));
+    SB2_TRY(knn_tc2_build_images(ctx, t1.sh, c.d_x, n_points, d, c.maxnorm, nullptr, 0, A1, t1.B, inv_s2, dnorm, c.maxnorm + 1));
+    t1.bound.dnorm = dnorm;
+    t1.bound.dmax = c.maxnorm + 1;
     // pilot: one wave of CTAs
-    const int64_t wave = s1.wave_rows(ctx);
+    const int64_t wave = (int64_t)ctx->prop.multiProcessorCount * TILE;
     const int64_t first = n_query >= 4 * wave ? wave : n_query;
-    SB2_TRY(t.evs->begin());
-    SB2_TRY(s1.sweep(ctx, A1, qt0, B1, n_points, first, list_m, cand_score, cand_idx, &t.issued_flops, true));
-    SB2_TRY(t.evs->end());
-    SB2_TRY(launch_rescore(ctx, list_m, sub, t.d_x, n_points, d, q0, 0, nullptr, first, k, cand_score, cand_idx, maxnorm, inv_s2, cq1,
-                           cn1, dnorm, maxnorm + 1, t.d_idx, t.d_dist, t.wq1, t.wub1, t.wcnt));
+    SB2_TRY(sweep_and_certify(c, t1, A1, 0, nullptr, first));
     done = first;
     if (first < n_query) {
       int64_t open1 = 0;
-      SB2_TRY(read_count(ctx, t.wcnt, &open1));
-      direct_split = open1 * 2 > first;
-      if (!direct_split) {
-        const int64_t rest = n_query - done;
-        SB2_TRY(t.evs->begin());
-        SB2_TRY(s1.sweep(ctx, A1, qt0 + done / TILE, B1, n_points, rest, list_m, cand_score + done * list_m,
-                         cand_idx + done * list_m, &t.issued_flops, true));
-        SB2_TRY(t.evs->end());
-        SB2_TRY(launch_rescore(ctx, list_m, sub, t.d_x, n_points, d, q0, done, nullptr, rest, k, cand_score + done * list_m,
-                               cand_idx + done * list_m, maxnorm, inv_s2, cq1, cn1, dnorm, maxnorm + 1, t.d_idx, t.d_dist, t.wq1, t.wub1, t.wcnt));
+      SB2_TRY(read_count(ctx, c.wcnt, &open1));
+      if (open1 * 2 <= first) {  // most pilot rows certified: tier 1 for the rest too
+        SB2_TRY(sweep_and_certify(c, t1, A1, done, nullptr, n_query - done));
         done = n_query;
       }
     }
   }
   if (done < n_query) {
     // split-precision sweep of the remaining rows, straight from the full image arrays
-    SB2_TRY(scr.alloc(&A3, s3.a_halves(n_points)));
-    SB2_TRY(scr.alloc(&B3, s3.b_halves(n_points)));
-    SB2_TRY(s3.build(ctx, t.d_x, n_points, d, maxnorm, nullptr, 0, A3, B3, inv_s2, nullptr, nullptr));
-    const int64_t rest = n_query - done;
-    SB2_TRY(t.evs->begin());
-    SB2_TRY(s3.sweep(ctx, A3, qt0 + done / TILE, B3, n_points, rest, list_m, cand_score + done * list_m,
-                     cand_idx + done * list_m, &t.issued_flops, true));
-    SB2_TRY(t.evs->end());
-    SB2_TRY(launch_rescore(ctx, list_m, sub, t.d_x, n_points, d, q0, done, nullptr, rest, k, cand_score + done * list_m,
-                           cand_idx + done * list_m, maxnorm, inv_s2, cq3, cn3, nullptr, nullptr, t.d_idx, t.d_dist, t.wq2, t.wub2, t.wcnt + 1));
+    __half* A3;
+    SB2_TRY(scr.alloc(&A3, knn_tc2_a_halves(t3.sh, n_points)));
+    SB2_TRY(scr.alloc(&t3.B, knn_tc2_b_halves(t3.sh, n_points)));
+    SB2_TRY(knn_tc2_build_images(ctx, t3.sh, c.d_x, n_points, d, c.maxnorm, nullptr, 0, A3, t3.B, inv_s2));
+    SB2_TRY(sweep_and_certify(c, t3, A3, done, nullptr, n_query - done));
   }
-  if (!split_only) {
-    // tier 2: gather the rows tier 1 left open and sweep them in split precision
-    SB2_TRY(read_count(ctx, t.wcnt, &t.n_resweep));
-    // a re-sweep occupies one CTA per 128 open rows for a whole pass over the candidates (a few ms at 1.3M points
-    // however few rows there are); the exact scan streams the whole data set once per ROW (~45 us each at
-    // 1.3M x 50 once HBM saturates), so it only wins for a handful of rows
-    int64_t scan_slots = 16;
-    if (const char* se = getenv("SB2_KNN_SCAN_SLOTS")) scan_slots = atoll(se);  // 0 forces the re-sweep (tests)
-    const int64_t n_resweep = t.n_resweep;
-    if (n_resweep > 0 && n_resweep <= scan_slots) {
-      knn_append_queue_kernel<<<(unsigned)ceil_div64(n_resweep, 256), 256, 0, st>>>(t.wq1, t.wub1, n_resweep, t.wq2, t.wub2, t.wcnt + 1);
-      SB2_LAUNCH_CHECK(ctx);
-    } else if (n_resweep > 0) {
-      if (!B3) {
-        SB2_TRY(scr.alloc(&B3, s3.b_halves(n_points)));
-        SB2_TRY(s3.build(ctx, t.d_x, n_points, d, maxnorm, nullptr, 0, nullptr, B3, inv_s2, nullptr, nullptr));
-      }
-      __half* Ag;
-      SB2_TRY(scr.alloc(&Ag, s3.a_halves(n_resweep)));
-      SB2_TRY(s3.build(ctx, t.d_x, n_resweep, d, maxnorm, t.wq1, q0, Ag, nullptr, inv_s2, nullptr, nullptr));
-      SB2_TRY(t.evs->begin());
-      // cold start: rows whose sampled threshold was too tight (fewer than k candidates beat it) must not fail twice
-      SB2_TRY(s3.sweep(ctx, Ag, 0, B3, n_points, n_resweep, list_m, cand_score, cand_idx, &t.issued_flops, false));
-      SB2_TRY(t.evs->end());
-      SB2_TRY(launch_rescore(ctx, list_m, sub, t.d_x, n_points, d, q0, 0, t.wq1, n_resweep, k, cand_score, cand_idx, maxnorm, inv_s2, cq3,
-                             cn3, nullptr, nullptr, t.d_idx, t.d_dist, t.wq2, t.wub2, t.wcnt + 1));
+  if (c.sw.split_only) return SB2_OK;
+  // tier 2: gather the rows tier 1 left open and sweep them in split precision
+  SB2_TRY(read_count(ctx, c.wcnt, &c.n_resweep));
+  // a re-sweep occupies one CTA per 128 open rows for a whole pass over the candidates (a few ms at 1.3M points
+  // however few rows there are); the exact scan streams the whole data set once per ROW (~45 us each at
+  // 1.3M x 50 once HBM saturates), so it only wins for a handful of rows
+  const int64_t n_resweep = c.n_resweep;
+  if (n_resweep > 0 && n_resweep <= c.sw.scan_slots) {
+    knn_append_queue_kernel<<<(unsigned)ceil_div64(n_resweep, 256), 256, 0, ctx->stream>>>(c.wq[0], c.wub[0], n_resweep, c.wq[1],
+                                                                                            c.wub[1], c.wcnt + 1);
+    SB2_LAUNCH_CHECK(ctx);
+  } else if (n_resweep > 0) {
+    if (!t3.B) {
+      SB2_TRY(scr.alloc(&t3.B, knn_tc2_b_halves(t3.sh, n_points)));
+      SB2_TRY(knn_tc2_build_images(ctx, t3.sh, c.d_x, n_points, d, c.maxnorm, nullptr, 0, nullptr, t3.B, inv_s2));
     }
+    __half* Ag;
+    SB2_TRY(scr.alloc(&Ag, knn_tc2_a_halves(t3.sh, n_resweep)));
+    SB2_TRY(knn_tc2_build_images(ctx, t3.sh, c.d_x, n_resweep, d, c.maxnorm, c.wq[0], c.q0, Ag, nullptr, inv_s2));
+    SB2_TRY(sweep_and_certify(c, t3, Ag, 0, c.wq[0], n_resweep));
   }
   return SB2_OK;
+}
+
+// The fp32 CUDA-core first pass (SB2_KNN_PASS1=ffma): 32 proposals per row; rows it cannot certify go to the exact scan
+int32_t ffma_pass(KnnCall& c) {
+  sb2_ctx* ctx = c.ctx;
+  cudaStream_t st = ctx->stream;
+  c.list_m = c.sub = LISTM;
+  SB2_TRY(c.scr->alloc(&c.cand_score, (size_t)c.n_query * LISTM));
+  SB2_TRY(c.scr->alloc(&c.cand_idx, (size_t)c.n_query * LISTM));
+  c.issued_flops = 2.0 * (double)c.n_query * (double)c.n_points * (double)c.d;
+  const double e = 1.5 * (double)(c.d + 2) * 5.9604644775390625e-08;
+  const int64_t n_tiles = ceil_div64(c.n_points, TILE), q_tiles = ceil_div64(c.n_query, TILE);
+  const size_t chunk_b = (size_t)(c.d + 1) * TILE * 4;
+  const size_t smem3 = chunk_b * 4 + 64, smem2 = chunk_b * 3 + 64;
+  const size_t lim = ctx->prop.sharedMemPerBlockOptin;
+  SB2_TRY(c.evs.begin());
+  if (smem3 <= lim) {
+    SB2_CUDA(cudaFuncSetAttribute(knn_pass1_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
+    knn_pass1_kernel<3><<<(unsigned)q_tiles, PASS1_THREADS, smem3, st>>>(c.Xt, c.d, n_tiles, c.q0 / TILE, c.n_query,
+                                                                         c.cand_score, c.cand_idx);
+  } else {
+    SB2_CHECK_ARG(smem2 <= lim, "d too large for shared memory");
+    SB2_CUDA(cudaFuncSetAttribute(knn_pass1_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+    knn_pass1_kernel<2><<<(unsigned)q_tiles, PASS1_THREADS, smem2, st>>>(c.Xt, c.d, n_tiles, c.q0 / TILE, c.n_query,
+                                                                         c.cand_score, c.cand_idx);
+  }
+  SB2_LAUNCH_CHECK(ctx);
+  SB2_TRY(c.evs.end());
+  return launch_rescore(c, Bound{e, e, nullptr, nullptr, nullptr, 1}, 0, nullptr, c.n_query);
 }
 
 }  // namespace
@@ -690,95 +747,43 @@ extern "C" int32_t sb2_knn_l2_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, con
   SB2_CHECK_ARG(q0 >= 0 && n_query >= 0 && q0 + n_query <= n_points, "query range");
   SB2_CHECK_ARG(q0 % TILE == 0, "q0 must be a multiple of 128");
   if (n_query == 0) return SB2_OK;
+  const KnnSwitches sw = knn_switches();
+  const bool use_tc = knn_tc2_supported(d) && !sw.ffma;
+  SB2_CHECK_ARG(use_tc || k <= LISTM - 2, "k > 30 needs the tensor-core pass (SB2_KNN_PASS1=ffma limits k to 30)");
   SB2_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   ScratchScope scr(ctx);
-  const int64_t n_tiles = ceil_div64(n_points, TILE);
-  const int64_t chunk_f = (int64_t)(d + 1) * TILE;
-  float* Xt;
-  unsigned int* maxnorm;
-  int32_t *wq1, *wq2;
-  double *wub1, *wub2;
-  unsigned long long* wcnt;  // [0] rows tier 1 left open, [1] rows for the exact scan
-  SB2_TRY(scr.alloc(&Xt, (size_t)(n_tiles * chunk_f)));
-  SB2_TRY(scr.alloc(&maxnorm, 4));
-  const char* force = getenv("SB2_KNN_PASS1");
-  const char* tiers = getenv("SB2_KNN_TIERS");
-  const bool use_tc = knn_tc2_supported(d) && !(force && strcmp(force, "ffma") == 0);
-  const bool split_only = tiers && strcmp(tiers, "3") == 0;
-  const char* list_env = getenv("SB2_KNN_LIST");
-  const bool big_list = list_env && (strcmp(list_env, "64") == 0 || strcmp(list_env, "128") == 0);
-  SB2_CHECK_ARG(use_tc || k <= LISTM - 2, "k > 30 needs the tensor-core pass (SB2_KNN_PASS1=ffma limits k to 30)");
-  SB2_TRY(scr.alloc(&wq1, (size_t)n_query));
-  SB2_TRY(scr.alloc(&wub1, (size_t)n_query));
-  SB2_TRY(scr.alloc(&wq2, (size_t)n_query));
-  SB2_TRY(scr.alloc(&wub2, (size_t)n_query));
-  SB2_TRY(scr.alloc(&wcnt, 2));
-  SB2_CUDA(cudaMemsetAsync(maxnorm, 0, 16, st));
-  SB2_CUDA(cudaMemsetAsync(wcnt, 0, 16, st));
-  {
-    size_t smem = (size_t)TILE * d * sizeof(float);
-    SB2_CUDA(cudaFuncSetAttribute(knn_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    knn_prep_kernel<<<(unsigned)n_tiles, 256, smem, st>>>(d_x, n_points, d, Xt, maxnorm);
-    SB2_LAUNCH_CHECK(ctx);
+  KnnCall c{ctx, &scr, sw, d_x, n_points, q0, n_query, d, k, d_idx, d_dist};
+  SB2_TRY(prep_points(ctx, scr, d_x, n_points, d, &c.Xt, &c.maxnorm));
+  for (int i = 0; i < 2; ++i) {
+    SB2_TRY(scr.alloc(&c.wq[i], (size_t)n_query));
+    SB2_TRY(scr.alloc(&c.wub[i], (size_t)n_query));
   }
-  EventPairs evs;
-  evs.on = info != nullptr;
-  evs.st = st;
-  double issued_flops = 0.0;
-  int64_t n_resweep = 0;
-  if (use_tc) {
-    TierState t{ctx, &scr, d_x, n_points, q0, n_query, d, k, maxnorm, wq1, wq2, wub1, wub2, wcnt, d_idx, d_dist, &evs};
-    SB2_TRY(tensor_tiers<SweepV2>(t, split_only, big_list));
-    issued_flops = t.issued_flops;
-    n_resweep = t.n_resweep;
-  } else {
-    float* cand_score;
-    int32_t* cand_idx;
-    SB2_TRY(scr.alloc(&cand_score, (size_t)n_query * LISTM));
-    SB2_TRY(scr.alloc(&cand_idx, (size_t)n_query * LISTM));
-    issued_flops = 2.0 * (double)n_query * (double)n_points * (double)d;
-    const double c = 1.5 * (double)(d + 2) * 5.9604644775390625e-08;
-    const int64_t q_tiles = ceil_div64(n_query, TILE);
-    const size_t chunk_b = (size_t)chunk_f * 4;
-    const size_t smem3 = chunk_b * 4 + 64, smem2 = chunk_b * 3 + 64;
-    const size_t lim = ctx->prop.sharedMemPerBlockOptin;
-    SB2_TRY(evs.begin());
-    if (smem3 <= lim) {
-      SB2_CUDA(cudaFuncSetAttribute(knn_pass1_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
-      knn_pass1_kernel<3><<<(unsigned)q_tiles, PASS1_THREADS, smem3, st>>>(Xt, d, n_tiles, q0 / TILE, n_query,
-                                                                           cand_score, cand_idx);
-    } else {
-      SB2_CHECK_ARG(smem2 <= lim, "d too large for shared memory");
-      SB2_CUDA(cudaFuncSetAttribute(knn_pass1_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-      knn_pass1_kernel<2><<<(unsigned)q_tiles, PASS1_THREADS, smem2, st>>>(Xt, d, n_tiles, q0 / TILE, n_query,
-                                                                           cand_score, cand_idx);
-    }
-    SB2_LAUNCH_CHECK(ctx);
-    SB2_TRY(evs.end());
-    SB2_TRY(launch_rescore(ctx, LISTM, LISTM, d_x, n_points, d, q0, 0, nullptr, n_query, k, cand_score, cand_idx, maxnorm, nullptr, c, c,
-                           nullptr, nullptr, d_idx, d_dist, wq2, wub2, wcnt + 1));
-  }
+  SB2_TRY(scr.alloc(&c.wcnt, 2));
+  SB2_CUDA(cudaMemsetAsync(c.wcnt, 0, 16, st));
+  c.evs.on = info != nullptr;
+  c.evs.st = st;
+  SB2_TRY(use_tc ? tensor_tiers(c) : ffma_pass(c));
   {
     const int grid = ctx->prop.multiProcessorCount * 4;
-    knn_fallback_kernel<<<grid, FB_THREADS, 0, st>>>(d_x, Xt, n_points, d, q0, k, wq2, wub2, wcnt + 1, d_idx, d_dist);
+    knn_fallback_kernel<<<grid, FB_THREADS, 0, st>>>(d_x, c.Xt, n_points, d, q0, k, c.wq[1], c.wub[1], c.wcnt + 1, d_idx, d_dist);
     SB2_LAUNCH_CHECK(ctx);
   }
   if (info) {
     unsigned long long h_cnt = 0;
     unsigned int h_bits = 0;
-    SB2_CUDA(cudaMemcpyAsync(&h_cnt, wcnt + 1, sizeof(h_cnt), cudaMemcpyDeviceToHost, st));
-    SB2_CUDA(cudaMemcpyAsync(&h_bits, maxnorm, sizeof(h_bits), cudaMemcpyDeviceToHost, st));
+    SB2_CUDA(cudaMemcpyAsync(&h_cnt, c.wcnt + 1, sizeof(h_cnt), cudaMemcpyDeviceToHost, st));
+    SB2_CUDA(cudaMemcpyAsync(&h_bits, c.maxnorm, sizeof(h_bits), cudaMemcpyDeviceToHost, st));
     SB2_CUDA(cudaStreamSynchronize(st));
     info->n_uncertified = (int64_t)h_cnt;
     float f;
     memcpy(&f, &h_bits, 4);
     info->max_norm = sqrtf(f);
-    info->pass1_ms = evs.total_ms();
+    info->pass1_ms = c.evs.total_ms();
     info->pass1_flops = 2.0 * (double)n_query * (double)n_points * (double)d;
-    info->pass1_issued_flops = issued_flops;
+    info->pass1_issued_flops = c.issued_flops;
     info->pass1_tensor = use_tc ? 2 : 0;
-    info->n_resweep = n_resweep;
+    info->n_resweep = c.n_resweep;
   }
   return SB2_OK;
 }
@@ -794,23 +799,15 @@ extern "C" int32_t sb2_knn_debug_proposals_f32(sb2_ctx* ctx, int64_t n_points, i
   SB2_CHECK_ARG(ctx && d_x && d_score && d_idx && h_meta, "null pointer");
   SB2_CHECK_ARG(terms == 1 || terms == 3, "terms must be 1 (fp16) or 3 (split fp16)");
   SB2_CHECK_ARG(n_points >= 1 && d >= 1 && d <= 150, "n_points / d");
+  const KnnSwitches sw = knn_switches();
   SB2_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   ScratchScope scr(ctx);
-  const int64_t n_tiles = ceil_div64(n_points, TILE);
   float* Xt;
   unsigned int* maxnorm;
+  SB2_TRY(prep_points(ctx, scr, d_x, n_points, d, &Xt, &maxnorm));
   float* inv_s2;
-  SB2_TRY(scr.alloc(&Xt, (size_t)(n_tiles * (d + 1) * TILE)));
-  SB2_TRY(scr.alloc(&maxnorm, 4));
   SB2_TRY(scr.alloc(&inv_s2, 4));
-  SB2_CUDA(cudaMemsetAsync(maxnorm, 0, 16, st));
-  {
-    size_t smem = (size_t)TILE * d * sizeof(float);
-    SB2_CUDA(cudaFuncSetAttribute(knn_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    knn_prep_kernel<<<(unsigned)n_tiles, 256, smem, st>>>(d_x, n_points, d, Xt, maxnorm);
-    SB2_LAUNCH_CHECK(ctx);
-  }
   KnnTc2Shape sh;
   SB2_CHECK_ARG(knn_tc2_shape(ctx, d, terms, false, &sh), "tile does not fit shared memory");
   __half *A, *B;
@@ -822,7 +819,7 @@ extern "C" int32_t sb2_knn_debug_proposals_f32(sb2_ctx* ctx, int64_t n_points, i
                                terms == 1 ? maxnorm + 1 : nullptr));
   const int list_m = 64;
   double fl = 0.0;
-  SB2_TRY(knn_tc2_sweep(ctx, sh, A, 0, B, n_points, n_points, list_m, d_score, d_idx, &fl, false));
+  SB2_TRY(knn_tc2_sweep(ctx, sw, sh, A, 0, B, n_points, n_points, list_m, d_score, d_idx, &fl));
   float h_inv = 0.0f;
   unsigned int h_bits[2] = {0, 0};
   SB2_CUDA(cudaMemcpyAsync(&h_inv, inv_s2, 4, cudaMemcpyDeviceToHost, st));

@@ -4,6 +4,24 @@
 
 #include "common.cuh"
 
+constexpr int EST_R = 6;           // chunk maxima an estimate keeps per (row, sub-list)
+constexpr int EST_STRIDE = 16;     // the estimate samples every 16th candidate tile
+
+// The kNN's run-time switches, read from the environment on every call by knn_switches (knn.cu).  The defaults are
+// what bench.py measures; every other setting gives the same neighbours.
+struct KnnSwitches {
+  bool ffma = false;            // SB2_KNN_PASS1=ffma: the fp32 CUDA-core first pass instead of the tensor-core tiers
+  bool split_only = false;      // SB2_KNN_TIERS=3: every row goes straight to the split-precision tier
+  bool big_list = false;        // SB2_KNN_LIST=64 or 128: 128-proposal lists for every k
+  bool cold = false;            // SB2_KNN_EST set to a value <= 0: every sweep starts cold
+  int est_stride = EST_STRIDE;  // SB2_KNN_EST=n > 0: the threshold estimate samples every n-th candidate tile
+  int est_rank = EST_R;         // SB2_KNN_EST_RANK=1..EST_R: which of the sampled chunk maxima seeds the sub-lists
+  int64_t scan_slots = 16;      // SB2_KNN_SCAN_SLOTS=n: up to n rows tier 1 leaves open go straight to the exact scan
+  bool pipe = true;             // SB2_KNN_PIPE=0 (false): the single-buffer consumer loop where the pipelined one could run
+  bool stamps = false;          // SB2_KNN_STAMPS=1: each sweep launch reports its consumers' cycle split on stderr
+  bool int_scan = true;         // SB2_KNN_SCAN=float (false): the float max tree in the fast path of the sweep's examination
+};
+
 // ---- tensor-core sweep (knn_tc2.cu): 128-query CTAs x 128-candidate tiles (wgmma N = 128), two consumer warpgroups,
 // four register-resident sub-lists per query row (one per column class of the accumulator fragment) ----
 struct KnnTc2Shape {
@@ -24,8 +42,9 @@ int32_t knn_tc2_build_images(sb2_ctx* ctx, const KnnTc2Shape& sh, const float* d
                              __half* Aimg, __half* Bimg, float* d_inv_s2, float* d_dnorm = nullptr,
                              unsigned int* d_dmax_bits = nullptr);
 // proposals: list_m (64 or 128) per query = four sub-lists of list_m/4, sub-list j in slots [j*list_m/4, (j+1)*list_m/4);
-// unused slots hold the sub-list's starting threshold (-inf for a cold start) and id -1
-int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnTc2Shape& sh, const __half* Aimg, int64_t a_tile0, const __half* Bimg,
-                      int64_t n_points, int64_t n_query, int list_m, float* cand_score, int32_t* cand_idx, double* issued_flops,
-                      bool estimate = true);
+// unused slots hold the sub-list's starting threshold (-inf for a cold start) and id -1.  Only a shape made with
+// want_estimate starts from a sampled threshold.
+int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnSwitches& sw, const KnnTc2Shape& sh, const __half* Aimg, int64_t a_tile0,
+                      const __half* Bimg, int64_t n_points, int64_t n_query, int list_m, float* cand_score, int32_t* cand_idx,
+                      double* issued_flops);
 void knn_tc2_error_coefs(const KnnTc2Shape& sh, double* c_q, double* c_n);

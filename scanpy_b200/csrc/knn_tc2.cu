@@ -31,7 +31,8 @@
 //   Sweep front: CTAs walk the candidate tiles cyclically, starting where the running CTAs currently are (g_knn2_front).
 #include <cuda_fp16.h>
 #include <float.h>
-#include <string.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "knn_internal.cuh"
@@ -55,9 +56,7 @@ constexpr int PROD_REGS = 40, CONS_REGS = 232;
 // fp16 at d = 50); other K axes take the single-buffer loop
 constexpr int PIPE_NKS0 = 4, PIPE_NKS1 = 10;
 static_assert(128 * PROD_REGS + 256 * CONS_REGS <= 65536 / THREADS_PIPE / 8 * 8 * THREADS_PIPE, "register file");
-constexpr int NSUB = 4;            // sub-lists per query row
-constexpr int EST_R = 6;           // chunk maxima an estimate keeps per (row, sub-list)
-constexpr int EST_STRIDE = 16;     // the estimate samples every 16th candidate tile
+constexpr int NSUB = 4;            // sub-lists per query row (EST_R, EST_STRIDE: knn_internal.cuh)
 constexpr uint32_t SBO = 128;              // bytes between 8-row groups (core matrices contiguous)
 constexpr uint32_t LBO = QM * 16;          // bytes between K-chunks of a 128-row image  [kc][row-group][8][8]
 static_assert(QM == CN, "query and candidate images share one layout");
@@ -641,35 +640,28 @@ int32_t knn_tc2_build_images(sb2_ctx* ctx, const KnnTc2Shape& sh, const float* d
 }
 
 namespace {
-template <int NG, int PNKS, bool STAMPS, bool ISCAN>
-cudaError_t launch2s(unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B, int64_t n_tiles,
-                     int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs,
-                     int32_t* ci, unsigned long long* stamps) {
-  cudaError_t e = cudaFuncSetAttribute(knn_sweep2_kernel<NG, PNKS, STAMPS, ISCAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
-  if (e != cudaSuccess) return e;
-  const int nks = sh.kpad / 16 / sh.nsplit;
-  knn_sweep2_kernel<NG, PNKS, STAMPS, ISCAN><<<grid, PNKS > 0 ? THREADS_PIPE : THREADS, sh.smem, st>>>(
-      A, B, nks, sh.nsplit, sh.nstage, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
-  return cudaSuccess;
-}
-template <int NG, int PNKS, bool ISCAN>
-cudaError_t launch2(unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B, int64_t n_tiles,
-                    int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query, int32_t n_points, float* cs,
-                    int32_t* ci, unsigned long long* stamps) {
-  if (stamps)
-    return launch2s<NG, PNKS, true, ISCAN>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
-  return launch2s<NG, PNKS, false, ISCAN>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
-}
-template <int NG, bool ISCAN>
-cudaError_t launch2_nks(bool pipe, unsigned grid, const KnnTc2Shape& sh, cudaStream_t st, const __half* A, const __half* B,
-                        int64_t n_tiles, int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query,
-                        int32_t n_points, float* cs, int32_t* ci, unsigned long long* stamps) {
-  const int nks = pipe ? sh.kpad / 16 : 0;   // knn_tc2_shape only sets pipe for nsplit = 1 and these two K axes
-  if (nks == PIPE_NKS0)
-    return launch2<NG, PIPE_NKS0, ISCAN>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
-  if (nks == PIPE_NKS1)
-    return launch2<NG, PIPE_NKS1, ISCAN>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
-  return launch2<NG, 0, ISCAN>(grid, sh, st, A, B, n_tiles, n_est, est_stride, est_rank, qtile0, n_query, n_points, cs, ci, stamps);
+// f(NG, PNKS, STAMPS, ISCAN) as std::integral_constants, the template arguments of knn_sweep2_kernel: NG = 2 for lists of
+// 64 proposals, 4 for 128; PNKS the pipelined loop's k-steps when pipe (knn_tc2_shape only sets it for nsplit = 1 and
+// these two K axes), else 0
+template <typename F>
+void with_sweep2(int list_m, bool iscan, bool pipe, int kpad, bool stamps, F&& f) {
+  using std::integral_constant;
+  const auto with_stamps = [&](auto ng, auto is, auto pnks) {
+    if (stamps) f(ng, pnks, std::true_type(), is);
+    else f(ng, pnks, std::false_type(), is);
+  };
+  const auto with_pnks = [&](auto ng, auto is) {
+    const int nks = pipe ? kpad / 16 : 0;
+    if (nks == PIPE_NKS0) with_stamps(ng, is, integral_constant<int, PIPE_NKS0>());
+    else if (nks == PIPE_NKS1) with_stamps(ng, is, integral_constant<int, PIPE_NKS1>());
+    else with_stamps(ng, is, integral_constant<int, 0>());
+  };
+  const auto with_scan = [&](auto ng) {
+    if (iscan) with_pnks(ng, std::true_type());
+    else with_pnks(ng, std::false_type());
+  };
+  if (list_m == 64) with_scan(integral_constant<int, 2>());
+  else with_scan(integral_constant<int, 4>());
 }
 
 // SB2_KNN_STAMPS=1: where the consumer warpgroups of one sweep spent their cycles, summed over all of them, and how
@@ -700,24 +692,22 @@ int32_t report_stamps(sb2_ctx* ctx, const KnnTc2Shape& sh, bool pipe, unsigned g
 }
 }  // namespace
 
-int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnTc2Shape& sh, const __half* Aimg, int64_t a_tile0, const __half* Bimg,
-                      int64_t n_points, int64_t n_query, int list_m, float* cand_score, int32_t* cand_idx, double* issued_flops,
-                      bool estimate) {
+int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnSwitches& sw, const KnnTc2Shape& sh, const __half* Aimg, int64_t a_tile0,
+                      const __half* Bimg, int64_t n_points, int64_t n_query, int list_m, float* cand_score, int32_t* cand_idx,
+                      double* issued_flops) {
   cudaStream_t st = ctx->stream;
   const int64_t n_tiles = ceil_div64(n_points, CN);
   const int64_t q_ctas = ceil_div64(n_query, QM);
   SB2_CHECK_ARG(list_m == 64 || list_m == 128, "list_m must be 64 or 128 (four sub-lists of 16 or 32)");
   // threshold estimate: the est_rank-th largest of the row's chunk maxima over every est_stride-th tile sits at about
   // rank est_rank * est_stride of the row
-  int64_t est_stride = EST_STRIDE, n_est = n_tiles / est_stride;
-  const char* est_env = getenv("SB2_KNN_EST");
-  if (est_env) est_stride = atoi(est_env) > 0 ? atoi(est_env) : est_stride, n_est = atoi(est_env) > 0 ? n_tiles / est_stride : 0;
-  if (n_tiles < 32 * est_stride || !estimate || !sh.est) n_est = 0;  // small problems / re-sweeps: cold start
+  const int64_t est_stride = sw.est_stride;
+  int64_t n_est = sw.cold ? 0 : n_tiles / est_stride;
+  if (n_tiles < 32 * est_stride || !sh.est) n_est = 0;  // small problems / split-precision sweeps: cold start
   // the sub-lists start at the est_rank-th largest of the row's sampled chunk maxima, rank ~96 of the row by default:
   // on the 1.3M x 50 benchmark (k = 15) every rank below 6 sends more rows to the split-precision re-sweep (rank 5:
   // 7x as many, rank 4: 46x) than it saves in insertions.  SB2_KNN_EST_RANK=1..6 picks another (tests, A/B timing).
-  int est_rank = EST_R;
-  if (const char* r_env = getenv("SB2_KNN_EST_RANK")) est_rank = atoi(r_env) >= 1 && atoi(r_env) <= EST_R ? atoi(r_env) : est_rank;
+  const int est_rank = sw.est_rank;
   if (issued_flops) *issued_flops += 2.0 * (double)(q_ctas * QM) * (double)((n_tiles + n_est) * CN) * (double)sh.kpad;
   const unsigned grid = (unsigned)q_ctas;
   const int32_t np = (int32_t)n_points;
@@ -726,23 +716,23 @@ int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnTc2Shape& sh, const __half* Aimg, i
     SB2_CUDA(cudaGetSymbolAddress(&fp, g_knn2_front));
     SB2_CUDA(cudaMemsetAsync(fp, 0, sizeof(unsigned long long), st));
   }
-  // SB2_KNN_PIPE=0 keeps the single-buffer consumer loop where the pipelined one could run (same results, A/B timing)
-  const char* pipe_env = getenv("SB2_KNN_PIPE");
-  const bool pipe = sh.pipe && !(pipe_env && strcmp(pipe_env, "0") == 0);
-  const char* stamps_env = getenv("SB2_KNN_STAMPS");
+  // SB2_KNN_PIPE=0 and SB2_KNN_SCAN=float give the same results (A/B timing)
+  const bool pipe = sh.pipe && sw.pipe;
   ScratchScope scr(ctx);
   unsigned long long* stamps = nullptr;
-  if (stamps_env && strcmp(stamps_env, "1") == 0) {
+  if (sw.stamps) {
     SB2_TRY(scr.alloc(&stamps, (size_t)grid * 2 * ST_N));
     SB2_CUDA(cudaMemsetAsync(stamps, 0, (size_t)grid * 2 * ST_N * sizeof(unsigned long long), st));
   }
-  // SB2_KNN_SCAN=float keeps the float max tree in the fast path of the examination (same results, A/B timing)
-  const char* scan_env = getenv("SB2_KNN_SCAN");
-  const bool iscan = !(scan_env && strcmp(scan_env, "float") == 0);
-  const auto launch = list_m == 64 ? (iscan ? launch2_nks<2, true> : launch2_nks<2, false>)
-                                   : (iscan ? launch2_nks<4, true> : launch2_nks<4, false>);
-  const cudaError_t le =
-      launch(pipe, grid, sh, st, Aimg, Bimg, n_tiles, n_est, est_stride, est_rank, a_tile0, n_query, np, cand_score, cand_idx, stamps);
+  cudaError_t le = cudaSuccess;
+  with_sweep2(list_m, sw.int_scan, pipe, sh.kpad, sw.stamps, [&](auto ng, auto pnks, auto st_on, auto iscan) {
+    le = cudaFuncSetAttribute(knn_sweep2_kernel<ng, pnks, st_on, iscan>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
+    if (le != cudaSuccess) return;
+    const int nks = sh.kpad / 16 / sh.nsplit;
+    knn_sweep2_kernel<ng, pnks, st_on, iscan><<<grid, pnks > 0 ? THREADS_PIPE : THREADS, sh.smem, st>>>(
+        Aimg, Bimg, nks, sh.nsplit, sh.nstage, n_tiles, n_est, est_stride, est_rank, a_tile0, n_query, np, cand_score, cand_idx,
+        stamps);
+  });
   SB2_CUDA(le);
   SB2_LAUNCH_CHECK(ctx);
   if (stamps) SB2_TRY(report_stamps(ctx, sh, pipe, grid, n_tiles + n_est, n_est, n_query, list_m, stamps));
