@@ -147,8 +147,146 @@ csr_gram_kernel(int64_t n, const int64_t* __restrict__ indptr, const int32_t* __
   }
 }
 
-// ---- Gram matrix, tiled variant (opt-in, SB2_GRAM_TILED=1; measured slower than the kernel above, see sb2_csr_gram) ----------
-// The kernel above issues one global fp64 RED per product (6.5e9 at 1.3M x 2000, ~195 G RED/s = 33 ms).
+// ---- Gram matrix by G rows (the default for column-sorted rows) -------------------------------------------------------
+// csr_gram_kernel issues one global fp64 RED per product: 6.5e9 at 1.3M x 2000, 82.1 ms on an H100 80GB HBM3 at 700 W,
+// which is the L2's atomic rate (~79 G RED/s).  Yet there are only g(g+1)/2 distinct cells.  Here a CTA owns row i of G
+// for one chunk of CSR rows: row i of G is the sum over the rows r holding column i of x_ri times the tail of row r that
+// starts at column i.  A warp walks one row tail at a time; within a tail the columns are distinct (strictly increasing),
+// so the lanes add into a warp-private fp64 copy of the G row in shared memory with plain loads and stores, no atomics
+// (a shared fp64 atomicAdd is a CAS loop on sm_90a).  At the end the CTA sums its warps' copies and flushes the row
+// segment [i, g) with one RED per non-zero cell.  Work items are chunk-major, so the CTAs resident at one time read row
+// tails of the same chunk and its CSR slice stays in the L2.
+//
+// The CSR positions holding column i within a chunk come from a counting sort keyed by (chunk, column): a count pass
+// (which also checks that every row's columns strictly increase inside [0, g); the caller falls back to csr_gram_kernel
+// otherwise), sb2_scan_i32_to_i64, and a scatter pass.  An entry of the sorted index packs the CSR position e (< 2^48) and
+// the row tail's length e1 - e (<= g < 2^16 for strictly increasing columns) into one 64-bit word.
+constexpr int GR_INDEX_ROWS = 1024;  // rows per CTA of the count and scatter passes; chunks are a multiple of it
+// The chunk trades the L2 footprint of its CSR slice (G itself takes 32 MB of the 50 MB at g = 2000) against the flush
+// (one RED per G cell per chunk).  csr_gram_rows_kernel at 1.3M x 2000 (H100 80GB HBM3, 700 W), whole sb2_csr_gram call:
+// 4 MB 49.0 ms, 8 MB 43.0, 16 MB 39.9, 32 MB 43.5, 64 MB 49.4.
+constexpr int64_t GR_CHUNK_BYTES = 16 << 20;
+__global__ void __launch_bounds__(256)
+gram_col_count_kernel(int64_t n, const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, int g,
+                      int64_t chunk_rows, int32_t* __restrict__ counts, int* __restrict__ flag) {
+  extern __shared__ int hist[];  // [g]
+  for (int c = threadIdx.x; c < g; c += blockDim.x) hist[c] = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const int64_t r0 = (int64_t)blockIdx.x * GR_INDEX_ROWS, r1 = min(n, r0 + GR_INDEX_ROWS);
+  bool bad = false;
+  for (int64_t row = r0 + (threadIdx.x >> 5); row < r1; row += blockDim.x >> 5) {
+    const int64_t e0 = indptr[row], e1 = indptr[row + 1];
+    int prev_last = -1;
+    for (int64_t e = e0; e < e1; e += 32) {
+      const bool on = e + lane < e1;
+      const int c = on ? indices[e + lane] : 0x7fffffff;
+      int pc = __shfl_up_sync(0xffffffffu, c, 1);
+      if (lane == 0) pc = prev_last;
+      prev_last = __shfl_sync(0xffffffffu, c, 31);
+      if (on) {
+        if (pc >= c || c >= g) bad = true;
+        else atomicAdd(&hist[c], 1);
+      }
+    }
+  }
+  if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(flag, 1);
+  __syncthreads();
+  int32_t* cnt = counts + (r0 / chunk_rows) * g;
+  for (int c = threadIdx.x; c < g; c += blockDim.x)
+    if (hist[c]) atomicAdd(&cnt[c], hist[c]);
+}
+// off[b] enters as the start of bucket b = chunk * g + column and leaves as its end (the start of bucket b + 1)
+__global__ void __launch_bounds__(256)
+gram_col_scatter_kernel(int64_t n, const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, int g,
+                        int64_t chunk_rows, int64_t* __restrict__ off, uint64_t* __restrict__ sorted) {
+  extern __shared__ int64_t base[];  // [g], then int rank[g]
+  int* rank = reinterpret_cast<int*>(base + g);
+  for (int c = threadIdx.x; c < g; c += blockDim.x) rank[c] = 0;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const int64_t r0 = (int64_t)blockIdx.x * GR_INDEX_ROWS, r1 = min(n, r0 + GR_INDEX_ROWS);
+  for (int64_t row = r0 + (threadIdx.x >> 5); row < r1; row += blockDim.x >> 5)
+    for (int64_t e = indptr[row] + lane, e1 = indptr[row + 1]; e < e1; e += 32) atomicAdd(&rank[indices[e]], 1);
+  __syncthreads();
+  int64_t* o = off + (r0 / chunk_rows) * g;
+  for (int c = threadIdx.x; c < g; c += blockDim.x) {
+    const int h = rank[c];
+    if (h) base[c] = (int64_t)atomicAdd(reinterpret_cast<unsigned long long*>(&o[c]), (unsigned long long)h);
+    rank[c] = 0;
+  }
+  __syncthreads();
+  for (int64_t row = r0 + (threadIdx.x >> 5); row < r1; row += blockDim.x >> 5) {
+    const int64_t e1 = indptr[row + 1];
+    for (int64_t e = indptr[row] + lane; e < e1; e += 32) {
+      const int c = indices[e];
+      sorted[base[c] + atomicAdd(&rank[c], 1)] = ((uint64_t)e << 16) | (uint64_t)(e1 - e);
+    }
+  }
+}
+// One CTA per bucket b = (chunk, gene i), chunk-major; blockDim.x / 32 warp copies of G[i, i:g) in shared memory.
+// end[b] is the end of bucket b in `sorted` (its start is end[b - 1]).
+__global__ void __launch_bounds__(512)
+csr_gram_rows_kernel(int g, const int64_t* __restrict__ end, const uint64_t* __restrict__ sorted,
+                     const int32_t* __restrict__ indices, const float* __restrict__ data, double* __restrict__ G) {
+  extern __shared__ double acc_all[];  // [warps][g]
+  const int i = (int)(blockIdx.x % g);
+  const int64_t b = (int64_t)(blockIdx.x / g) * g + i;
+  const int64_t s = b > 0 ? end[b - 1] : 0, t = end[b];
+  if (s == t) return;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
+  const int w = g - i;  // cells [i, g) of the G row; acc[c - i] for column c
+  double* acc = acc_all + (size_t)warp * g;
+  for (int k = lane; k < w; k += 32) acc[k] = 0.0;
+  __syncwarp();
+  for (int64_t q0 = s + (int64_t)warp * 32; q0 < t; q0 += (int64_t)warps * 32) {
+    const int m = (int)min((int64_t)32, t - q0);
+    int64_t p = 0;
+    int len = 0;
+    double vi = 0.0;
+    if (lane < m) {
+      const uint64_t e = sorted[q0 + lane];
+      p = (int64_t)(e >> 16);
+      len = (int)(e & 0xffff);
+      vi = (double)data[p];
+    }
+    // the first 64 entries of the next row tail are loaded while the current one is added up
+    int c0 = 0, c1 = 0;
+    float x0 = 0.0f, x1 = 0.0f;
+    {
+      const int64_t pq = __shfl_sync(0xffffffffu, p, 0);
+      const int lq = __shfl_sync(0xffffffffu, len, 0);
+      if (lane < lq) { c0 = indices[pq + lane]; x0 = data[pq + lane]; }
+      if (lane + 32 < lq) { c1 = indices[pq + lane + 32]; x1 = data[pq + lane + 32]; }
+    }
+    for (int q = 0; q < m; ++q) {
+      const int64_t pq = __shfl_sync(0xffffffffu, p, q);
+      const int lq = __shfl_sync(0xffffffffu, len, q);
+      const double vq = __shfl_sync(0xffffffffu, vi, q);
+      const int64_t pn = __shfl_sync(0xffffffffu, p, (q + 1) & 31);
+      const int ln = q + 1 < m ? __shfl_sync(0xffffffffu, len, (q + 1) & 31) : 0;
+      int n0 = 0, n1 = 0;
+      float y0 = 0.0f, y1 = 0.0f;
+      if (lane < ln) { n0 = indices[pn + lane]; y0 = data[pn + lane]; }
+      if (lane + 32 < ln) { n1 = indices[pn + lane + 32]; y1 = data[pn + lane + 32]; }
+      if (lane < lq) acc[c0 - i] += vq * (double)x0;
+      if (lane + 32 < lq) acc[c1 - i] += vq * (double)x1;
+      for (int k = lane + 64; k < lq; k += 32) acc[indices[pq + k] - i] += vq * (double)data[pq + k];
+      __syncwarp();  // the next tail may add into cells this one's lanes touched
+      c0 = n0; c1 = n1; x0 = y0; x1 = y1;
+    }
+  }
+  __syncthreads();
+  double* Gi = G + (size_t)i * g + i;
+  for (int k = threadIdx.x; k < w; k += blockDim.x) {
+    double v = 0.0;
+    for (int c = 0; c < warps; ++c) v += acc_all[(size_t)c * g + k];
+    if (v != 0.0) atomicAdd(&Gi[k], v);
+  }
+}
+
+// ---- Gram matrix, tiled variant (opt-in, SB2_GRAM_TILED=1; measured slower than csr_gram_kernel, see sb2_csr_gram) --------
+// csr_gram_kernel issues one global fp64 RED per product (6.5e9 at 1.3M x 2000, ~79 G RED/s = 82 ms on an H100).
 // Here the g columns are cut into NB blocks of GT_W; a CTA owns one tile pair (bi <= bj) of G for a contiguous range of
 // rows and keeps that GT_W x GT_W fp64 tile in shared memory (128 KB): for every row, the entries falling into blocks bi
 // and bj (contiguous, rows are column-sorted; their positions come from a per-row block-offset table built once) are
@@ -1126,6 +1264,58 @@ int32_t sb2_spmm_csr_t(sb2_ctx* ctx, int64_t n, int32_t g, int32_t l, const int6
   return launch_spmm_t(ctx, n, g, l, d_indptr, d_indices, d_data, d_y, Zc, d_z);
 }
 
+// G (zeroed, upper triangle) by csr_gram_rows_kernel; *done stays false when a row is not strictly column-sorted inside
+// [0, g) or the warp copies of a G row do not fit, and the caller then runs csr_gram_kernel.
+static int32_t gram_by_rows(sb2_ctx* ctx, int64_t n, int g, const int64_t* d_indptr, const int32_t* d_indices,
+                            const float* d_data, double* d_gram, bool* done) {
+  // warp copies of G[i, i:g) per CTA: as many as let two CTAs share an SM, else as many as one CTA can hold, at least 2.
+  // At 1.3M x 2000 (H100, 700 W) two CTAs of 7 warps took 39.9 ms, one of 8 warps 61.1, one of 14 43.9, three of 4 43.6.
+  const size_t copy = sizeof(double) * (size_t)g;
+  const size_t per_sm = ctx->prop.sharedMemPerMultiprocessor, per_cta = ctx->prop.sharedMemPerBlockOptin;
+  int warps = (int)std::min<size_t>(16, (per_sm / 2 - ctx->prop.reservedSharedMemPerBlock) / copy);
+  if (warps < 2) warps = (int)std::min<size_t>(16, per_cta / copy);
+  if (warps < 2) return SB2_OK;
+  int64_t nnz = 0;
+  SB2_CUDA(cudaMemcpyAsync(&nnz, d_indptr + n, sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+  SB2_CUDA(cudaStreamSynchronize(ctx->stream));
+  // row chunks whose indices + data take ~GR_CHUNK_BYTES, so that the slice the resident CTAs read stays in the L2
+  const int64_t row_bytes = std::max<int64_t>(1, 8 * nnz / n);
+  const int64_t chunk_rows = GR_INDEX_ROWS * std::max<int64_t>(1, GR_CHUNK_BYTES / row_bytes / GR_INDEX_ROWS);
+  const int64_t n_chunks = ceil_div64(n, chunk_rows), nb = n_chunks * g;
+  if (nb > 0x7fffffff) return SB2_OK;
+  ScratchScope scr(ctx);
+  int32_t* counts;
+  int64_t* off;
+  uint64_t* sorted;
+  int* flag;
+  SB2_TRY(scr.alloc(&counts, (size_t)nb));
+  SB2_TRY(scr.alloc(&off, (size_t)nb + 1));
+  SB2_TRY(scr.alloc(&sorted, (size_t)nnz));
+  SB2_TRY(scr.alloc(&flag, 1));
+  SB2_CUDA(cudaMemsetAsync(counts, 0, sizeof(int32_t) * nb, ctx->stream));
+  SB2_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), ctx->stream));
+  const unsigned index_ctas = (unsigned)ceil_div64(n, GR_INDEX_ROWS);
+  const size_t count_smem = sizeof(int) * g, scatter_smem = (sizeof(int64_t) + sizeof(int)) * g;
+  const size_t rows_smem = copy * warps;
+  SB2_CUDA(cudaFuncSetAttribute(gram_col_count_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)count_smem));
+  SB2_CUDA(cudaFuncSetAttribute(gram_col_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scatter_smem));
+  SB2_CUDA(cudaFuncSetAttribute(csr_gram_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)rows_smem));
+  gram_col_count_kernel<<<index_ctas, 256, count_smem, ctx->stream>>>(n, d_indptr, d_indices, g, chunk_rows, counts, flag);
+  SB2_LAUNCH_CHECK(ctx);
+  int hflag = 0;
+  SB2_CUDA(cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  SB2_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (hflag) return SB2_OK;
+  SB2_TRY(sb2_scan_i32_to_i64(ctx, counts, nb, off));
+  gram_col_scatter_kernel<<<index_ctas, 256, scatter_smem, ctx->stream>>>(n, d_indptr, d_indices, g, chunk_rows, off,
+                                                                          sorted);
+  SB2_LAUNCH_CHECK(ctx);
+  csr_gram_rows_kernel<<<(unsigned)nb, 32 * warps, rows_smem, ctx->stream>>>(g, off, sorted, d_indices, d_data, d_gram);
+  SB2_LAUNCH_CHECK(ctx);
+  *done = true;
+  return SB2_OK;
+}
+
 int32_t sb2_csr_gram(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_indptr, const int32_t* d_indices,
                      const float* d_data, double* d_gram) {
   SB2_CHECK_ARG(ctx && d_indptr && d_gram, "null pointer");
@@ -1133,10 +1323,12 @@ int32_t sb2_csr_gram(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_indptr
   SB2_CUDA(cudaMemsetAsync(d_gram, 0, sizeof(double) * (size_t)g * g, ctx->stream));
   bool done = false;
   const int NB = (int)ceil_div64(g, GT_W);
-  // The tiled kernel is opt-in (SB2_GRAM_TILED=1); the default issues one global fp64 RED per product, which the L2
-  // retires, while the tiled kernel's shared-memory fp64 atomicAdd is a CAS loop (ATOMS.CAST.SPIN.64) behind a chain of
-  // dependent global loads (block offsets -> indices/data).  Both give the same result up to the fp64 summation order.
+  // The tiled kernel is opt-in (SB2_GRAM_TILED=1): its shared-memory fp64 atomicAdd is a CAS loop (ATOMS.CAST.SPIN.64)
+  // behind a chain of dependent global loads (block offsets -> indices/data).  Without it, csr_gram_rows_kernel runs
+  // where it applies and csr_gram_kernel (one global fp64 RED per product) elsewhere.  All give the same result up to
+  // the fp64 summation order.
   static const bool use_tiled = getenv("SB2_GRAM_TILED") != nullptr;
+  if (n > 0 && !use_tiled) SB2_TRY(gram_by_rows(ctx, n, g, d_indptr, d_indices, d_data, d_gram, &done));
   if (n >= 2048 && g >= 64 && NB <= 63 && use_tiled) {
     // tiled kernel: needs column-sorted rows (checked while the block-offset table is built)
     ScratchScope scr(ctx);
