@@ -410,6 +410,64 @@ int32_t sb2_dense_col_stats(sb2_ctx* ctx, int64_t n, int32_t g, const void* d_x,
 int32_t sb2_dense_scale(sb2_ctx* ctx, int64_t n, int32_t g, void* d_x, int32_t is_f64, const double* d_mean,
                         const double* d_std, const uint8_t* d_mask, int32_t has_max, double max_value);
 
+/* ---- sc.pp.harmony_integrate (src/scanpy/preprocessing/_harmony/core.py; csrc/harmony.cu) ----
+ * Z, R, X and the outputs are row-major [n x d] / [n x k], float32 (is_f64 = 0) or float64; d_y, d_pen, d_w and every
+ * sum are fp64.  d_codes [n x keys] int32 holds each cell's marginal code per key, in [0, n_codes).  A cell list d_idx
+ * (int64, NULL: the identity) names the rows a call works on.  Sums have no floating-point atomics: per-CTA partials
+ * fold in CTA order, and the CTA split depends only on the shapes, so equal inputs give equal bits.
+ * sb2_harmony_normalize <- _normalize_rows_l2: d_out[i] = d_x[i] / max(||d_x[i]||, 1e-12).
+ * sb2_harmony_wsums     <- d_out[g][c][j] = Σ_{rows of group g} w(i, c) * [z_i | 1][j], fp64 [groups x k x (d+1)].  The
+ *                          call's rows are d_idx[0 .. h_bounds[groups]) (row i = d_idx[p]), group g owning positions
+ *                          h_bounds[g] .. h_bounds[g+1] (host array).  w: d_r[i][c] (mode 0), 1 where d_labels[i] == c
+ *                          (mode 1, float64 Z only), or 1 with k = 1 (mode 2).
+ * sb2_harmony_step      <- one block of the clustering: for each listed cell, log r = term (1 - z·y_c) + Σ_keys
+ *                          d_pen[code][c] (d_pen NULL: no penalty), minus its max, exp, divided by max(Σ, 1e-12), stored
+ *                          to d_r; d_ent[i] = Σ_c r̂ log(r̂ + 1e-12) with r̂ = r / max(Σ r, 1e-12).
+ * sb2_harmony_code_sums <- d_out fp64 [(n_codes + 1) x k]: row b the sum of d_r over the listed cells with code b for
+ *                          any key, row n_codes the sum over all listed cells.
+ * sb2_harmony_oe_update <- o += sign * sums[b], e += sign * pr_b[b] * sums[n_codes], then d_pen[b][c] = theta[b] *
+ *                          (log(e + 1) - log(o + e + 1)) (stabilized) or theta[b] * (log(e + 1) - log(o + 1)).
+ * sb2_harmony_sum       <- *d_out = Σ d_v[0 .. n).
+ * sb2_harmony_center / sb2_harmony_kpp_search / sb2_harmony_kpp_dists / sb2_harmony_labels <- sklearn's KMeans on
+ *                          the rows of Z: d_xc = z - d_mean and d_xx = ||d_xc||²; for each uniform d_u[t], the first i
+ *                          with cumsum(d_v)[i] >= d_u[t] (n - 1 if none); for each candidate row d_ids[t],
+ *                          d_dist[t][i] = min(d_closest[i], max(-2 xc_i·xc_c + ||xc_c||² + xx_i, 0)) (d_closest NULL: no
+ *                          min) and d_pot[t] = Σ_i d_dist[t][i]; d_labels[i] = argmin_c ||c||² - 2 xc_i·c (first),
+ *                          *d_changed = 1 if any label differs from d_old.
+ * sb2_harmony_apply     <- the correction: for each group g of rows (as in wsums) with code tuple d_gcodes[g] [keys],
+ *                          z_i = x_i - Σ_c r_ic Σ_keys d_w[c][code + 1] (d_w fp64 [k x (n_codes + 1) x d]) to d_zhat,
+ *                          and z_i / max(||z_i||, 1e-12) to d_znorm. */
+#define SB2_HARMONY_MAX_K 128
+#define SB2_HARMONY_MAX_D 128
+#define SB2_HARMONY_MAX_CODES 128
+#define SB2_HARMONY_MAX_TUPLES 65536
+#define SB2_HARMONY_MAX_TRIALS 8
+int32_t sb2_harmony_normalize(sb2_ctx* ctx, int64_t n, int32_t d, int32_t is_f64, const void* d_x, void* d_out);
+int32_t sb2_harmony_wsums(sb2_ctx* ctx, int32_t groups, const int64_t* h_bounds, const int64_t* d_idx, int32_t d,
+                          int32_t k, int32_t is_f64, const void* d_z, int32_t mode, const void* d_r,
+                          const int32_t* d_labels, double* d_out);
+int32_t sb2_harmony_step(sb2_ctx* ctx, int64_t rows, const int64_t* d_idx, int32_t d, int32_t k, int32_t is_f64,
+                         const void* d_z, const double* d_y, int32_t keys, const int32_t* d_codes, const double* d_pen,
+                         double term, void* d_r, double* d_ent);
+int32_t sb2_harmony_code_sums(sb2_ctx* ctx, int64_t rows, const int64_t* d_idx, int32_t k, int32_t is_f64,
+                              const void* d_r, int32_t keys, const int32_t* d_codes, int32_t n_codes, double* d_out);
+int32_t sb2_harmony_oe_update(sb2_ctx* ctx, int32_t n_codes, int32_t k, double sign, const double* d_sums,
+                              const double* d_pr_b, const double* d_theta, int32_t stabilized, double* d_o, double* d_e,
+                              double* d_pen);
+int32_t sb2_harmony_sum(sb2_ctx* ctx, int64_t n, const double* d_v, double* d_out);
+int32_t sb2_harmony_center(sb2_ctx* ctx, int64_t n, int32_t d, int32_t is_f64, const void* d_z, const double* d_mean,
+                           double* d_xc, double* d_xx);
+int32_t sb2_harmony_kpp_search(sb2_ctx* ctx, int64_t n, const double* d_v, int32_t trials, const double* d_u,
+                               int64_t* d_ids);
+int32_t sb2_harmony_kpp_dists(sb2_ctx* ctx, int64_t n, int32_t d, const double* d_xc, const double* d_xx,
+                              int32_t trials, const int64_t* d_ids, const double* d_closest, double* d_dist,
+                              double* d_pot);
+int32_t sb2_harmony_labels(sb2_ctx* ctx, int64_t n, int32_t d, int32_t k, const double* d_xc, const double* d_centers,
+                           const int32_t* d_old, int32_t* d_labels, int32_t* d_changed);
+int32_t sb2_harmony_apply(sb2_ctx* ctx, int32_t groups, const int64_t* h_bounds, const int64_t* d_idx, int32_t d,
+                          int32_t k, int32_t is_f64, int32_t keys, const int32_t* d_gcodes, int32_t n_codes,
+                          const double* d_w, const void* d_x, const void* d_r, void* d_zhat, void* d_znorm);
+
 #ifdef __cplusplus
 }
 #endif

@@ -138,6 +138,24 @@ SIGNATURES = {
     "sb2_combat_adjust": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p]),
+    "sb2_harmony_normalize": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p]),
+    "sb2_harmony_wsums": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_int32,
+                                    c_void_p, c_void_p, c_void_p]),
+    "sb2_harmony_step": (c_int32, [c_void_p, c_int64, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_int32,
+                                   c_void_p, c_void_p, c_double, c_void_p, c_void_p]),
+    "sb2_harmony_code_sums": (c_int32, [c_void_p, c_int64, c_void_p, c_int32, c_int32, c_void_p, c_int32, c_void_p,
+                                        c_int32, c_void_p]),
+    "sb2_harmony_oe_update": (c_int32, [c_void_p, c_int32, c_int32, c_double, c_void_p, c_void_p, c_void_p, c_int32,
+                                        c_void_p, c_void_p, c_void_p]),
+    "sb2_harmony_sum": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p]),
+    "sb2_harmony_center": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "sb2_harmony_kpp_search": (c_int32, [c_void_p, c_int64, c_void_p, c_int32, c_void_p, c_void_p]),
+    "sb2_harmony_kpp_dists": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                                        c_void_p, c_void_p]),
+    "sb2_harmony_labels": (c_int32, [c_void_p, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
+                                     c_void_p]),
+    "sb2_harmony_apply": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p,
+                                    c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "sb2_autocorr_sums": (c_int32, [c_void_p, c_int64, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
