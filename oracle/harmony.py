@@ -58,14 +58,22 @@ def kmeans_start(x: np.ndarray, n_clusters: int, random_state: np.random.RandomS
         sums = np.zeros_like(centers)
         np.add.at(sums, labels, xc)
         empty = np.flatnonzero(counts == 0)
-        if empty.size:  # sklearn: the points farthest from their centres start the empty clusters
-            far = np.argpartition(((xc - centers[labels]) ** 2).sum(axis=1), -empty.size)[: -empty.size - 1 : -1]
+        dist = ((xc - centers[labels]) ** 2).sum(axis=1) if empty.size else None
+        # sklearn: the points farthest from their centres start the empty clusters, unless every point sits on its
+        # centre (fewer distinct points than clusters); an empty cluster's centre is then 0
+        if empty.size and dist.max() > 0:
+            far = np.argpartition(dist, -empty.size)[: -empty.size - 1 : -1]
             for k, i in zip(empty, far):
                 sums[labels[i]] -= xc[i]
                 sums[k] = xc[i]
                 counts[k] = 1.0
                 counts[labels[i]] -= 1.0
-        new = np.where(counts[:, None] > 0, sums * (1.0 / np.maximum(counts, 1.0))[:, None], sums)
+        avg = sums * (1.0 / np.maximum(counts, 1.0))[:, None]
+        # sklearn's _average_centers: a cluster still empty takes the centre of the largest one as the loop over the
+        # clusters leaves it, averaged when it comes earlier and still a sum when it comes later
+        big = int(np.argmax(counts))
+        later = (np.arange(len(counts)) > big)[:, None]
+        new = np.where(counts[:, None] > 0, avg, np.where(later, avg[big], sums[big]))
         shift = ((new - centers) ** 2).sum()
         centers = new
         if np.array_equal(labels, labels_old) or shift <= tol:

@@ -268,15 +268,24 @@ def kmeans_start(dev: _Dev, n_clusters: int, rs: np.random.RandomState, dtype, m
         s = s[0]
         sums, counts = s[:, :d].copy(), s[:, d].copy()
         empty = np.flatnonzero(counts == 0)
-        if empty.size:  # sklearn: the points farthest from their centres start the empty clusters
+        if empty.size:
             h_xc, lab = _ops._to_host(xc, labels[1])
-            far = np.argpartition(((h_xc - centers[lab]) ** 2).sum(axis=1), -empty.size)[: -empty.size - 1 : -1]
+            dist = ((h_xc - centers[lab]) ** 2).sum(axis=1)
+        # sklearn: the points farthest from their centres start the empty clusters, unless every point sits on its
+        # centre (fewer distinct points than clusters); an empty cluster's centre is then 0
+        if empty.size and dist.max() > 0:
+            far = np.argpartition(dist, -empty.size)[: -empty.size - 1 : -1]
             for k, i in zip(empty, far):
                 sums[lab[i]] -= h_xc[i]
                 sums[k] = h_xc[i]
                 counts[k] = 1.0
                 counts[lab[i]] -= 1.0
-        new = np.where(counts[:, None] > 0, sums * (1.0 / np.maximum(counts, 1.0))[:, None], sums)
+        avg = sums * (1.0 / np.maximum(counts, 1.0))[:, None]
+        # sklearn's _average_centers: a cluster still empty takes the centre of the largest one as the loop over the
+        # clusters leaves it, averaged when it comes earlier and still a sum when it comes later
+        big = int(np.argmax(counts))
+        later = (np.arange(len(counts)) > big)[:, None]
+        new = np.where(counts[:, None] > 0, avg, np.where(later, avg[big], sums[big]))
         shift = ((new - centers) ** 2).sum()
         centers = new
         if not flag[0] or shift <= tol:

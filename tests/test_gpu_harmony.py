@@ -8,7 +8,7 @@ import pytest
 from oracle import harmony as oh
 from scanpy_b200 import _harmony as hm
 from scanpy_b200._compat import MiniAnnData
-from test_harmony_cpu import case_args, golden_cases, pbmc68k
+from test_harmony_cpu import case_args, golden_cases, pbmc68k, repeated_points
 
 pytestmark = pytest.mark.gpu
 
@@ -67,22 +67,39 @@ ORACLE_CASES = {
     "one_block": dict(block_proportion=1.0),
     "pruning": dict(batch_prune_threshold=0.2, n_clusters=8),
     "tau": dict(tau=3, sigma=0.2),
+    # real shapes: groups above CHUNK_ROWS = 2048 cells and K·(d+1) = 5,100 outputs (3 slices) in wsums
+    "default_k": dict(n=12_000, d=50, levels=(5,), n_clusters=None),
+    # more than 48 KB of shared memory in step, apply and wsums
+    "wide_basis": dict(n=8000, d=100, levels=(4,), n_clusters=100),
+    # the caps: K = d = 128 and 128 marginal codes (code_sums at 132 KB of shared memory), the multi-key solve
+    "caps": dict(n=6000, d=128, levels=(64, 64), n_clusters=128),
+    # 120 codes, thousands of code tuples of 1 to 3 cells
+    "many_tuples": dict(n=20_000, d=30, levels=(40, 40, 40), n_clusters=20),
 }
+SHAPED = ["default_k", "wide_basis", "caps", "many_tuples"]
 
 
 def oracle_case(name, dtype):
+    """A case's data, codes, k-means centres and arguments.  `n`, `d` and `levels` (per key) shape the data; the
+    schedule is NEG's, so every case runs max_iter_harmony x max_iter_clustering iterations."""
     spec = dict(ORACLE_CASES[name])
     keys = spec.pop("keys", 1)
     unused = spec.pop("unused", False)
-    x, obs, _ = synthetic(n_batches=(4, 3)[:keys], unused=unused)
+    n, d = spec.pop("n", 1501), spec.pop("d", 20)
+    x, obs, _ = synthetic(n=n, d=d, n_batches=spec.pop("levels", (4, 3)[:keys]), unused=unused)
     codes, n_levels = hm.get_batch_codes(obs, list(obs.columns))
     args = full_args(n_clusters=6, max_iter_harmony=3, max_iter_clustering=5, **NEG)
     args.update(spec)
     x = x.astype(dtype)
     z64 = x.astype(np.float64)
     z64 /= np.linalg.norm(z64, axis=1, keepdims=True)
-    centers, _ = oh.kmeans_start(z64, args["n_clusters"], hm.spawn_random_state(np.random.default_rng(11)))
+    k = args["n_clusters"] or max(int(min(100, n / 30)), 2)
+    centers, _ = oh.kmeans_start(z64, k, hm.spawn_random_state(np.random.default_rng(11)))
     return x, codes, n_levels, centers, args
+
+
+def schedule(args):
+    return [args["max_iter_clustering"]] * args["max_iter_harmony"]
 
 
 @pytest.mark.parametrize("name", list(ORACLE_CASES))
@@ -90,12 +107,12 @@ def test_device_matches_oracle_f64(name):
     x, codes, n_levels, centers, args = oracle_case(name, np.float64)
     z, its = device_fit(x, codes, n_levels, centers=centers, rng=11, **args)
     want, wits = oh.harmony(x, codes, n_levels, centers=centers, rng=11, **args)
-    assert its == wits == [5, 5, 5]
+    assert its == wits == schedule(args)
     err = np.abs(z - want).max() / np.abs(x).max()
     assert err <= 1e-8, err
 
 
-@pytest.mark.parametrize("name", ["harmony2", "harmony1", "two_keys", "pruning"])
+@pytest.mark.parametrize("name", ["harmony2", "harmony1", "two_keys", "pruning", *SHAPED])
 def test_device_matches_oracle_f32(name):
     """float32 stores Z, R and the output in float32 and does the dots and the exponent in float32.  A float32 dot of
     unit rows is off by ~1e-7; times |term| = 2 / sigma = 20 that moves log r by ~2e-6, and r, the correction weights
@@ -103,7 +120,8 @@ def test_device_matches_oracle_f32(name):
     allows for that growth; a schedule or indexing fault moves the result by more than 1e-2 x max|x|."""
     x, codes, n_levels, centers, args = oracle_case(name, np.float32)
     z, its = device_fit(x, codes, n_levels, centers=centers, rng=11, **args)
-    want, _ = oh.harmony(x.astype(np.float64), codes, n_levels, centers=centers, rng=11, **args)
+    want, wits = oh.harmony(x.astype(np.float64), codes, n_levels, centers=centers, rng=11, **args)
+    assert its == wits == schedule(args)
     assert z.dtype == np.float32
     err = np.abs(z - want).max() / np.abs(x).max()
     assert err <= 1e-4, err
@@ -120,6 +138,84 @@ def test_kmeans_start_matches_sklearn(n_clusters):
     z = x / np.linalg.norm(x, axis=1, keepdims=True)
     want = KMeans(n_clusters, random_state=hm.spawn_random_state(np.random.default_rng(0)), max_iter=25).fit(z)
     np.testing.assert_allclose(got, want.cluster_centers_, rtol=0, atol=1e-10)
+
+
+def _dev_kmeans(z, n_clusters, seed):
+    dev = hm._Dev(z, np.zeros((len(z), 1), dtype=np.int32), 1)
+    return hm.kmeans_start(dev, n_clusters, hm.spawn_random_state(np.random.default_rng(seed)), z.dtype)
+
+
+@pytest.mark.parametrize("d", [50, 128])
+@pytest.mark.parametrize("n_clusters", [33, 100, 128])
+@pytest.mark.parametrize("n", [1025, 20_000])
+def test_kmeans_start_matches_oracle_at_real_shapes(n, n_clusters, d):
+    """Clusters on every lane of `labels_kernel` (up to four per lane), Lloyd sums over several CHUNK_ROWS chunks and
+    the segmented k-means++ search (n > 1024), against the oracle's k-means start, and live sklearn at one shape."""
+    x, _, _ = synthetic(n=n, d=d, n_batches=(4,), seed=n + d)
+    got = _dev_kmeans(x, n_clusters, 5)
+    z = x / np.linalg.norm(x, axis=1, keepdims=True)
+    want, _ = oh.kmeans_start(z, n_clusters, hm.spawn_random_state(np.random.default_rng(5)))
+    np.testing.assert_allclose(got, want, rtol=0, atol=1e-10)
+    if (n, n_clusters, d) == (20_000, 100, 50):
+        from sklearn.cluster import KMeans
+
+        sk = KMeans(n_clusters, random_state=hm.spawn_random_state(np.random.default_rng(5)), max_iter=25).fit(z)
+        np.testing.assert_allclose(got, sk.cluster_centers_, rtol=0, atol=1e-10)
+
+
+def test_kmeans_start_with_fewer_distinct_points_than_clusters():
+    """k-means++ at a potential of exactly 0, then Lloyd with 24 clusters that stay empty: sklearn leaves them
+    unrelocated (every point sits on its centre) and places them at the largest cluster's centre."""
+    from sklearn.cluster import KMeans
+    from sklearn.exceptions import ConvergenceWarning
+
+    x = repeated_points()
+    assert len(np.unique(x, axis=0)) == 40
+    got = _dev_kmeans(x, 64, 2)
+    with pytest.warns(ConvergenceWarning, match="distinct clusters"):
+        sk = KMeans(64, random_state=hm.spawn_random_state(np.random.default_rng(2)), max_iter=25).fit(x)
+    want, _ = oh.kmeans_start(x, 64, hm.spawn_random_state(np.random.default_rng(2)))
+    np.testing.assert_array_equal(want, sk.cluster_centers_)
+    np.testing.assert_allclose(got, sk.cluster_centers_, rtol=0, atol=1e-12)
+
+
+def _f32_start_case(name):
+    if name == "pbmc68k":
+        x, obs, _ = pbmc68k()
+        return x.astype(np.float32), obs, "bulk_labels"
+    x, obs, _ = synthetic(n=12_000, d=50, n_batches=(5,))
+    return x.astype(np.float32), obs, "key0"
+
+
+@pytest.mark.parametrize("name", ["pbmc68k", "default_k"])
+def test_public_float32_call_against_scanpys_float32_start(name):
+    """scanpy runs sklearn's KMeans on the float32 rows, in float32; the device runs its k-means start in float64 on
+    the float32 rows.  The public float32 call against the oracle started from sklearn's float32 centres, with the
+    float32 bar of the oracle tests.  Printed next to it: the same device fit from sklearn's centres, which separates
+    the start's share of the error from the float32 schedule's."""
+    from sklearn.cluster import KMeans
+
+    from scanpy_b200 import pp
+
+    x, obs, key = _f32_start_case(name)
+    adata = MiniAnnData(np.zeros((len(x), 1), dtype=np.float32), obs=obs, obsm={"X_pca": x})
+    pp.harmony_integrate(adata, key, dtype=np.float32, rng=0)
+    got = adata.obsm["X_pca_harmony"]
+    assert got.dtype == np.float32
+    z = x / np.maximum(np.linalg.norm(x, axis=1, keepdims=True), np.float32(1e-12))
+    k = max(int(min(100, len(x) / 30)), 2)
+    sk = KMeans(k, random_state=hm.spawn_random_state(np.random.default_rng(0)), max_iter=25).fit(z).cluster_centers_
+    assert sk.dtype == np.float32
+    codes, n_levels = hm.get_batch_codes(obs, key)
+    want, wits = oh.harmony(x.astype(np.float64), codes, n_levels, centers=sk, rng=0)
+    scale = np.abs(x).max()
+    err = np.abs(got - want).max() / scale
+    from_sk, its = device_fit(x, codes, n_levels, centers=sk, rng=0, **full_args())
+    err_sk = np.abs(from_sk - want).max() / scale
+    centres = np.abs(_dev_kmeans(x, k, 0) - sk).max()
+    print(f"[{name}] float32 public call vs oracle from sklearn float32 centres: {err:.2e} x max|x|; the device fit "
+          f"from those centres: {err_sk:.2e} (iterations {its} vs {wits}); device start vs sklearn's: {centres:.2e}")
+    assert err <= 1e-4, err
 
 
 def _measure(x, base, norm):

@@ -63,6 +63,28 @@ def test_oracle_kmeans_start_matches_sklearn(n_clusters):
     np.testing.assert_allclose(got, want, rtol=0, atol=1e-12)
 
 
+def repeated_points(n=5000, d=64, distinct=40, seed=0):
+    """`distinct` points repeated to n rows: ± pairs of sign vectors / 8, so the rows have norm 1, the mean is 0 and
+    every squared distance is exact in float64 whatever the order of its sums.  k-means++ then reaches a potential of
+    exactly 0, and Lloyd sees clusters without points."""
+    rng = np.random.default_rng(seed)
+    s = rng.choice([-0.125, 0.125], size=(distinct // 2, d))
+    pts = np.vstack([s, -s])
+    return pts[rng.permutation(np.resize(np.arange(distinct), n))]
+
+
+def test_oracle_kmeans_start_with_fewer_distinct_points_than_clusters():
+    """Zero potential in k-means++ and clusters that Lloyd leaves empty, where sklearn skips the relocation and warns."""
+    from sklearn.cluster import KMeans
+    from sklearn.exceptions import ConvergenceWarning
+
+    x = repeated_points()
+    with pytest.warns(ConvergenceWarning, match="distinct clusters"):
+        want = KMeans(64, random_state=hm.spawn_random_state(np.random.default_rng(2)), max_iter=25).fit(x)
+    got, _ = oh.kmeans_start(x, 64, hm.spawn_random_state(np.random.default_rng(2)))
+    np.testing.assert_array_equal(got, want.cluster_centers_)
+
+
 def test_golden_kmeans_centres_are_sklearns():
     """The recorded centres are sklearn's from the spawned stream of rng=0 on the normalised X_pca."""
     x, _, g = pbmc68k()
