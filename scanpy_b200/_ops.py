@@ -225,89 +225,10 @@ def _pca_stream_solve(ctx, n: int, g: int, stats, gram, n_comps: int, seed: int)
     return out, proj, shift, l.value
 
 
-OVERLAP_MIN_NNZ = 1 << 24   # below ~16.7M stored entries the upload is too short to be worth pipelining
-
-
-def _pca_csr_overlapped(ctx, x, n_comps: int, seed: int, n_chunks: int = 8):
-    """Gram-route PCA of a HOST scipy CSR with the upload hidden behind the first pass over the data: the CSR arrays go up
-    in `n_chunks` row ranges on a side stream, and as each range lands the compute stream adds its column statistics and
-    Gram matrix (sb2_pca_stream_accumulate_f32 - the out-of-core entry point, pointed at the resident arrays).  The
-    projection then runs over the whole resident matrix.  Same arithmetic as solver 1 up to the fp64 summation order.
-    OPT-IN (SB2_PCA_OVERLAP=1): at the bench workload the upload is a small part of the step, so the plain upload stays
-    the default."""
-    torch = _torch()
-    n, g = x.shape
-    nnz = int(x.nnz)
-    main = torch.cuda.current_stream()
-    side = _side_stream()
-    indptr64 = np.asarray(x.indptr, dtype=np.int64)
-    h_idx = torch.from_numpy(np.ascontiguousarray(x.indices, dtype=np.int32))
-    h_dat = torch.from_numpy(np.ascontiguousarray(x.data, dtype=np.float32))
-    d_indptr = torch.empty(n + 1, dtype=torch.int64, device="cuda")
-    d_indices = torch.empty(nnz, dtype=torch.int32, device="cuda")
-    d_data = torch.empty(nnz, dtype=torch.float32, device="cuda")
-    stats = torch.zeros(2 * g, dtype=torch.float64, device="cuda")
-    gram = torch.zeros((g, g), dtype=torch.float64, device="cuda")
-    cuts = np.unique(np.r_[0, np.searchsorted(indptr64, np.linspace(0, nnz, n_chunks + 1)[1:-1]), n]).astype(np.int64)
-    side.wait_stream(main)   # the fresh allocations above may recycle blocks still in use on the compute stream
-    pending = []
-    with torch.cuda.stream(side):
-        for r0, r1 in zip(cuts[:-1], cuts[1:]):
-            lo, hi = int(indptr64[r0]), int(indptr64[r1])
-            ip = torch.from_numpy(indptr64[r0:r1 + 1] - lo)
-            parts = []
-            for dst, src in ((d_indices[lo:hi], h_idx[lo:hi]), (d_data[lo:hi], h_dat[lo:hi])):
-                if src.numel() and not src.is_pinned():
-                    src = src.pin_memory()
-                dst.copy_(src, non_blocking=True)
-                parts.append(src)
-            ipp = ip.pin_memory()
-            d_ip = ipp.to("cuda", non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(side)
-            pending.append((int(r0), int(r1), lo, hi, d_ip, ev, (parts, ipp)))
-        hp = torch.from_numpy(indptr64)
-        hp = hp if hp.is_pinned() else hp.pin_memory()
-        d_indptr.copy_(hp, non_blocking=True)
-        ev_all = torch.cuda.Event()
-        ev_all.record(side)
-    TRANSFER["h2d"] += nnz * 8 + (n + 1) * 8 + (n + len(pending)) * 8
-    for r0, r1, lo, hi, d_ip, ev, _keep in pending:
-        main.wait_event(ev)
-        d_ip.record_stream(main)
-        check(ctx.lib.sb2_pca_stream_accumulate_f32(ctx.handle, r1 - r0, g, ptr(d_ip), ptr(d_indices[lo:hi]) if hi > lo else ptr(d_indices),
-                                                    ptr(d_data[lo:hi]) if hi > lo else ptr(d_data), ptr(stats), ptr(gram)))
-    out, proj, shift, l = _pca_stream_solve(ctx, n, g, stats, gram, n_comps, seed)
-    main.wait_event(ev_all)
-    out["X_pca"] = torch.empty((n, n_comps), dtype=torch.float32, device="cuda")
-    check(ctx.lib.sb2_pca_stream_project_f32(ctx.handle, n, g, ptr(d_indptr), ptr(d_indices), ptr(d_data), n_comps, l, ptr(proj),
-                                             ptr(shift), ptr(out["X_pca"])))
-    for t in (d_indptr, d_indices, d_data):
-        t.record_stream(side)
-    return out
-
-
-_SIDE = {}
-
-
-def _side_stream():
-    torch = _torch()
-    dev = torch.cuda.current_device()
-    if dev not in _SIDE:
-        _SIDE[dev] = torch.cuda.Stream(device=dev)
-    return _SIDE[dev]
-
-
 def pca_csr(x, n_comps: int, *, solver: int = 0, max_iter: int = 0, tol: float = 0.0, seed: int = 0, ctx=None):
     """Top-n_comps PCA of a scipy CSR matrix; host arrays out (X_pca float32 [n,k], components float32 [k,g])."""
-    import os
-
     ctx = ctx or _abi.default_context()
     n, g = x.shape
-    min_nnz = int(os.environ.get("SB2_PCA_OVERLAP_MIN_NNZ", OVERLAP_MIN_NNZ))
-    if (solver == 1 and max_iter == 0 and tol == 0.0 and x.nnz >= min_nnz and getattr(ctx, "n_ranks", 1) == 1
-            and g >= 64 and os.environ.get("SB2_PCA_OVERLAP", "0") == "1"):
-        return _download_pca(_pca_csr_overlapped(ctx, x, n_comps, seed))
     d_indptr, d_indices, d_data = csr_to_device(x)
     return _download_pca(pca_csr_device(ctx, d_indptr, d_indices, d_data, n, g, n_comps, solver=solver, max_iter=max_iter,
                                         tol=tol, seed=seed))

@@ -12,7 +12,11 @@
 //                          read as one 128..512 B segment per non-zero     bytes: 8*nnz + 4*n*l
 //   spmm_csr_t_kernel      Z += X^T*Y, warp per row, (l/4) lanes per non-zero issue one
 //                          RED.ADD.F32x4 each into one of 8 replicated fp32 copies of Z (L2 resident)
-//   csr_gram_kernel        G += x_r x_r^T (upper triangle), warp per row, fp64 REDs into L2-resident G
+//   csr_gram_rows_kernel   G = X^T X (upper triangle), a CTA per (row chunk, G row i): the row tails holding column i,
+//                          found through a column index built by gram_col_count_kernel and gram_col_scatter_kernel, add
+//                          into per-warp fp64 copies of G[i, i:g) in shared memory, flushed with one RED per cell
+//   csr_gram_kernel        G += x_r x_r^T (upper triangle), warp per row, fp64 REDs into L2-resident G; for unsorted
+//                          rows and for g whose warp copies do not fit in shared memory
 //   small dense fp64 helpers (g x l blocks, l <= 128): A^T B, A*M, C*V, residual norms.
 //   rr_jacobi_kernel       the l x l Rayleigh-Ritz eigenproblem for l <= 64, one CTA (fp64).
 // Host side (C++ in this file): the block subspace iteration, CholeskyQR2 with an eigen-based
@@ -285,100 +289,6 @@ csr_gram_rows_kernel(int g, const int64_t* __restrict__ end, const uint64_t* __r
   }
 }
 
-// ---- Gram matrix, tiled variant (opt-in, SB2_GRAM_TILED=1; measured slower than csr_gram_kernel, see sb2_csr_gram) --------
-// csr_gram_kernel issues one global fp64 RED per product (6.5e9 at 1.3M x 2000, ~79 G RED/s = 82 ms on an H100).
-// Here the g columns are cut into NB blocks of GT_W; a CTA owns one tile pair (bi <= bj) of G for a contiguous range of
-// rows and keeps that GT_W x GT_W fp64 tile in shared memory (128 KB): for every row, the entries falling into blocks bi
-// and bj (contiguous, rows are column-sorted; their positions come from a per-row block-offset table built once) are
-// multiplied pairwise and added with shared-memory atomics; the tile is flushed to G with one global RED per non-zero
-// tile entry at the end.  CTAs are ordered row-range-major, so the CTAs resident at any time walk the same rows and the
-// CSR streams through the L2 once per wave instead of once per tile pair.
-constexpr int GT_W = 128;
-constexpr int GT_THREADS = 512;
-// boff[row * (NB+1) + b] = number of entries of the row with column < b * GT_W (uint16: a row holds < 65536 entries);
-// *flag |= 1 if a row is not column-sorted or too long (the caller then falls back to the first-generation kernel)
-__global__ void __launch_bounds__(256)
-gram_block_offsets_kernel(int64_t n, const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices, int NB,
-                          uint16_t* __restrict__ boff, int* __restrict__ flag) {
-  const int lane = threadIdx.x & 31;
-  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= n) return;
-  const int64_t e0 = indptr[row], e1 = indptr[row + 1];
-  if (e1 - e0 >= 65536) { if (lane == 0) atomicOr(flag, 1); }
-  int lo = 0, hi = 0;  // counts for b = lane and b = lane + 32
-  int prev_last = -1;
-  bool bad = false;
-  for (int64_t e = e0; e < e1; e += 32) {
-    const bool on = e + lane < e1;
-    const int c = on ? indices[e + lane] : 0x7fffffff;
-    int pc = __shfl_up_sync(0xffffffffu, c, 1);
-    if (lane == 0) pc = prev_last;
-    if (on && pc > c) bad = true;
-    prev_last = __shfl_sync(0xffffffffu, c, 31);
-    const int blk = on ? c / GT_W : 0x7fffffff;
-    for (int b = 1; b <= NB; ++b) {
-      const int x = __popc(__ballot_sync(0xffffffffu, on && blk < b));
-      if (b == lane) lo += x;
-      if (b == lane + 32) hi += x;
-    }
-  }
-  if (__any_sync(0xffffffffu, bad) && lane == 0) atomicOr(flag, 1);
-  uint16_t* o = boff + (size_t)row * (NB + 1);
-  if (lane <= NB) o[lane] = (uint16_t)lo;
-  if (lane + 32 <= NB) o[lane + 32] = (uint16_t)hi;
-}
-__global__ void __launch_bounds__(GT_THREADS, 1)
-csr_gram_tiles_kernel(int64_t n, const int64_t* __restrict__ indptr, const int32_t* __restrict__ indices,
-                      const float* __restrict__ data, const uint16_t* __restrict__ boff, int NB, int n_pairs,
-                      const int2* __restrict__ pair_tab, int64_t rows_per_range, double* __restrict__ G, int g) {
-  extern __shared__ double tile[];  // [GT_W][GT_W]
-  const int pair = blockIdx.x % n_pairs;
-  const int64_t range = blockIdx.x / n_pairs;
-  const int bi = pair_tab[pair].x, bj = pair_tab[pair].y;
-  for (int t = threadIdx.x; t < GT_W * GT_W; t += GT_THREADS) tile[t] = 0.0;
-  __syncthreads();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int64_t r0 = range * rows_per_range, r1 = min(n, r0 + rows_per_range);
-  const bool diag = bi == bj;
-  for (int64_t row = r0 + warp; row < r1; row += GT_THREADS / 32) {
-    const uint16_t* bo = boff + (size_t)row * (NB + 1);
-    const int a0 = bo[bi], p = (int)bo[bi + 1] - a0;
-    const int b0 = bo[bj], q = (int)bo[bj + 1] - b0;
-    if (p <= 0 || q <= 0) continue;
-    const int64_t base = indptr[row];
-    for (int ia = 0; ia < p; ia += 32) {
-      const int na = min(32, p - ia);
-      int ca = 0;
-      double va = 0.0;
-      if (lane < na) { ca = indices[base + a0 + ia + lane] - bi * GT_W; va = (double)data[base + a0 + ia + lane]; }
-      for (int ib = 0; ib < q; ib += 32) {
-        if (diag && ib + 31 < ia) continue;  // every (i, j) of this chunk pair has j < i
-        const int nb = min(32, q - ib);
-        int cb = 0;
-        double vb = 0.0;
-        if (lane < nb) { cb = indices[base + b0 + ib + lane] - bj * GT_W; vb = (double)data[base + b0 + ib + lane]; }
-        const int np = na * nb;
-        for (int t0 = 0; t0 < np; t0 += 32) {
-          const int t = t0 + lane;
-          const bool on = t < np;
-          const int i = on ? t / nb : 0, j = on ? t - i * nb : 0;
-          const int ci = __shfl_sync(0xffffffffu, ca, i), cj = __shfl_sync(0xffffffffu, cb, j);
-          const double vi = __shfl_sync(0xffffffffu, va, i), vj = __shfl_sync(0xffffffffu, vb, j);
-          // diagonal tiles: each unordered pair of entries once (positions i <= j; sorted columns => ci <= cj)
-          if (on && (!diag || ia + i <= ib + j)) atomicAdd(&tile[ci * GT_W + cj], vi * vj);
-        }
-      }
-    }
-  }
-  __syncthreads();
-  for (int t = threadIdx.x; t < GT_W * GT_W; t += GT_THREADS) {
-    const double v = tile[t];
-    if (v != 0.0) {
-      const int r = bi * GT_W + t / GT_W, c = bj * GT_W + t % GT_W;
-      if (r < g && c < g) atomicAdd(&G[(size_t)r * g + c], v);
-    }
-  }
-}
 __global__ void mirror_upper_kernel(double* __restrict__ G, int g) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (int64_t)g * g) return;
@@ -1321,57 +1231,10 @@ int32_t sb2_csr_gram(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_indptr
   SB2_CHECK_ARG(ctx && d_indptr && d_gram, "null pointer");
   SB2_CUDA(cudaSetDevice(ctx->device));
   SB2_CUDA(cudaMemsetAsync(d_gram, 0, sizeof(double) * (size_t)g * g, ctx->stream));
+  // csr_gram_rows_kernel where it applies (column-sorted rows, two warp copies of a G row fit in shared memory),
+  // csr_gram_kernel (one global fp64 RED per product) elsewhere; both give the same result up to the fp64 summation order
   bool done = false;
-  const int NB = (int)ceil_div64(g, GT_W);
-  // The tiled kernel is opt-in (SB2_GRAM_TILED=1): its shared-memory fp64 atomicAdd is a CAS loop (ATOMS.CAST.SPIN.64)
-  // behind a chain of dependent global loads (block offsets -> indices/data).  Without it, csr_gram_rows_kernel runs
-  // where it applies and csr_gram_kernel (one global fp64 RED per product) elsewhere.  All give the same result up to
-  // the fp64 summation order.
-  static const bool use_tiled = getenv("SB2_GRAM_TILED") != nullptr;
-  if (n > 0 && !use_tiled) SB2_TRY(gram_by_rows(ctx, n, g, d_indptr, d_indices, d_data, d_gram, &done));
-  if (n >= 2048 && g >= 64 && NB <= 63 && use_tiled) {
-    // tiled kernel: needs column-sorted rows (checked while the block-offset table is built)
-    ScratchScope scr(ctx);
-    uint16_t* boff;
-    int* flag;
-    int2* pair_tab;
-    SB2_TRY(scr.alloc(&boff, (size_t)n * (NB + 1)));
-    SB2_TRY(scr.alloc(&flag, 4));
-    const int n_pairs = NB * (NB + 1) / 2;
-    SB2_TRY(scr.alloc(&pair_tab, (size_t)n_pairs));
-    std::vector<int2> hp;
-    hp.reserve(n_pairs);
-    for (int bi = 0; bi < NB; ++bi)
-      for (int bj = bi; bj < NB; ++bj) hp.push_back(make_int2(bi, bj));
-    SB2_CUDA(cudaMemcpyAsync(pair_tab, hp.data(), sizeof(int2) * n_pairs, cudaMemcpyHostToDevice, ctx->stream));
-    SB2_CUDA(cudaMemsetAsync(flag, 0, 16, ctx->stream));
-    gram_block_offsets_kernel<<<(unsigned)ceil_div64(n, 8), 256, 0, ctx->stream>>>(n, d_indptr, d_indices, NB, boff, flag);
-    SB2_LAUNCH_CHECK(ctx);
-    int hflag = 0;
-    SB2_CUDA(cudaMemcpyAsync(&hflag, flag, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    SB2_CUDA(cudaStreamSynchronize(ctx->stream));  // also keeps hp alive until the copy has run
-    if (hflag == 0) {
-      // row ranges: enough CTAs for ~8 waves, a whole number of waves where possible, ranges of >= 1024 rows
-      const int sms = ctx->prop.multiProcessorCount;
-      int64_t best_s = 1;
-      double best_fill = 0.0;
-      const int64_t s_max = std::max<int64_t>(1, n / 1024);
-      const int64_t s0 = std::max<int64_t>(1, std::min<int64_t>(s_max, (int64_t)8 * sms / n_pairs));
-      for (int64_t sr = s0; sr <= std::min<int64_t>(s_max, s0 + 16); ++sr) {
-        const double ctas = (double)n_pairs * (double)sr;
-        const double fill = ctas / (ceil(ctas / sms) * sms);
-        if (fill > best_fill + 1e-9) { best_fill = fill; best_s = sr; }
-      }
-      const int64_t rows_per_range = ceil_div64(n, best_s);
-      const int64_t n_ranges = ceil_div64(n, rows_per_range);
-      const size_t smem = sizeof(double) * GT_W * GT_W;
-      SB2_CUDA(cudaFuncSetAttribute(csr_gram_tiles_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      csr_gram_tiles_kernel<<<(unsigned)(n_pairs * n_ranges), GT_THREADS, smem, ctx->stream>>>(
-          n, d_indptr, d_indices, d_data, boff, NB, n_pairs, pair_tab, rows_per_range, d_gram, g);
-      SB2_LAUNCH_CHECK(ctx);
-      done = true;
-    }
-  }
+  if (n > 0) SB2_TRY(gram_by_rows(ctx, n, g, d_indptr, d_indices, d_data, d_gram, &done));
   if (n > 0 && !done) {
     csr_gram_kernel<<<(unsigned)ceil_div64(n, 8), 256, 0, ctx->stream>>>(n, d_indptr, d_indices, d_data, d_gram, g);
     SB2_LAUNCH_CHECK(ctx);

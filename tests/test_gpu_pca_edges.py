@@ -9,12 +9,7 @@ case here runs such a branch on both operators where the route allows and compar
 first column with variance <= 1e-9 of the largest on null components; variance and variance_ratio to 1e-5.  A result that
 reports `converged` must meet that bar.  Each case prints its measured errors next to the bars.
 """
-import json
-import os
-import subprocess
-import sys
 import warnings
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -27,7 +22,6 @@ from scanpy_b200._synth import synth_scipy
 
 pytestmark = pytest.mark.gpu
 
-ROOT = Path(__file__).resolve().parent.parent
 CAP = {1: 4000, 0: 300}   # default iteration caps of the Gram and SpMM routes
 
 
@@ -307,88 +301,3 @@ def test_building_blocks_awkward_rows(l):
     np.testing.assert_allclose(s2.cpu().numpy(), np.asarray(xd.multiply(xd).sum(axis=0)).ravel(), rtol=1e-12)
     print(f"\n[building blocks l={l}] X B {np.abs(y.cpu().numpy() - y_ref).max():.2e}, "
           f"X^T Y {np.abs(z.cpu().numpy() - z_ref).max() / np.abs(z_ref).max():.2e} (relative to max)")
-
-
-# ------------------------------------------------------------------------------------------ tiled Gram
-_TILED_SCRIPT = r"""
-import json, sys
-import numpy as np
-import torch
-from scipy import sparse
-import scanpy_b200 as sb
-from scanpy_b200 import _ops
-
-f = np.load(sys.argv[1])
-ctx = sb._abi.default_context()
-res = {}
-for name in f["names"]:
-    x = sparse.csr_matrix((f[name + "_data"], f[name + "_indices"], f[name + "_indptr"]), shape=tuple(f[name + "_shape"]))
-    n, g = x.shape
-    dp, di, dd = _ops.csr_to_device(x)
-    gram = torch.empty((g, g), dtype=torch.float64, device="cuda")
-    torch.cuda.synchronize()
-    l0 = ctx.lib.sb2_ctx_launch_count(ctx.handle)
-    sb._abi.check(ctx.lib.sb2_csr_gram(ctx.handle, n, g, _ops.ptr(dp), _ops.ptr(di), _ops.ptr(dd), _ops.ptr(gram)))
-    torch.cuda.synchronize()
-    launches = ctx.lib.sb2_ctx_launch_count(ctx.handle) - l0
-    xd = x.astype(np.float64)
-    ref = torch.from_numpy((xd.T @ xd).toarray()).cuda()
-    rel = float(((gram - ref).abs() / ref.abs().clamp_min(1e-300)).max())
-    res[str(name)] = dict(launches=int(launches), rel=rel, zero_ok=bool(((ref == 0) == (gram == 0)).all()))
-    del gram, ref
-x = sparse.csr_matrix((f["pca_data"], f["pca_indices"], f["pca_indptr"]), shape=tuple(f["pca_shape"]))
-out = _ops.pca_csr(x, int(f["pca_k"]), solver=1)
-np.savez(sys.argv[2], X_pca=out["X_pca"], components=out["components"], variance=out["variance"])
-print("RESULT " + json.dumps(res))
-"""
-
-
-def _tiled_matrix(n, g, nnz_row, seed, unsorted=False):
-    rs = np.random.RandomState(seed)
-    ind, ptr = [], [0]
-    for r in range(n):
-        c = np.sort(rs.choice(g, min(g, nnz_row), replace=False))
-        if unsorted and r == n // 2:
-            c = c[::-1].copy()
-        ind.append(c)
-        ptr.append(ptr[-1] + len(c))
-    ind = np.concatenate(ind).astype(np.int32)
-    data = rs.uniform(0.1, 3.0, len(ind)).astype(np.float32)
-    return sparse.csr_matrix((data, ind, np.asarray(ptr, np.int64)), shape=(n, g))
-
-
-def test_tiled_gram_opt_in(tmp_path):
-    # SB2_GRAM_TILED=1 is read once per process, so the opt-in kernel runs in a child process: column-sorted rows at
-    # g from one block (64) to the 63-block limit (8064), one column past it (plain kernel), and one unsorted row (plain
-    # kernel); every result against float64 X^T X
-    cases = {f"g{g}": _tiled_matrix(2048 if g > 2000 else 4096, g, 40 if g > 2000 else 24, g) for g in (64, 127, 128, 129, 2000)}
-    cases["g8064"] = _tiled_matrix(2048, 8064, 40, 8064)
-    cases["g8065"] = _tiled_matrix(2048, 8065, 40, 8065)
-    cases["unsorted"] = _tiled_matrix(4096, 500, 30, 5, unsorted=True)
-    x_pca, _ = synth_scipy(4096, 2000, n_clusters=8, r=40, seed=30)
-    k = 30
-    arrays = dict(names=np.array(list(cases)), pca_k=k)
-    for name, x in list(cases.items()) + [("pca", x_pca)]:
-        arrays.update({f"{name}_data": x.data, f"{name}_indices": x.indices, f"{name}_indptr": x.indptr.astype(np.int64),
-                       f"{name}_shape": np.array(x.shape)})
-    np.savez(tmp_path / "in.npz", **arrays)
-    env = dict(os.environ, SB2_GRAM_TILED="1", PYTHONPATH=os.pathsep.join([str(ROOT)] + sys.path))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    p = subprocess.run([sys.executable, *flags, "-c", _TILED_SCRIPT, str(tmp_path / "in.npz"), str(tmp_path / "out.npz")],
-                       env=env, cwd=ROOT, capture_output=True, text=True, timeout=900)
-    assert p.returncode == 0, p.stderr[-4000:]
-    res = json.loads(next(line for line in p.stdout.splitlines() if line.startswith("RESULT "))[7:])
-    print("\n[tiled Gram] " + ", ".join(f"{k}: rel {v['rel']:.1e} launches {v['launches']}" for k, v in res.items()) + " (bar 1e-12)")
-    for name, r in res.items():
-        assert r["rel"] <= 1e-12 and r["zero_ok"], (name, r)
-    # block offsets + tiles + mirror where the tiled kernel applies; plain kernel + mirror past 63 blocks
-    for name in ("g64", "g127", "g128", "g129", "g2000", "g8064", "unsorted"):
-        assert res[name]["launches"] == 3, (name, res[name])
-    assert res["g8065"]["launches"] == 2
-    # the whole PCA on the tiled Gram matrix == the default kernel's
-    tiled = np.load(tmp_path / "out.npz")
-    plain = _ops.pca_csr(x_pca, k, solver=1)
-    np.testing.assert_allclose(tiled["variance"], plain["variance"], rtol=1e-10)
-    scale = np.abs(plain["X_pca"]).max(axis=0)
-    assert (np.abs(tiled["X_pca"] - plain["X_pca"]) / scale).max() < 1e-6
-    np.testing.assert_allclose(tiled["components"], plain["components"], atol=1e-6)

@@ -367,29 +367,6 @@ def test_pca_chunked_from_an_on_disk_zarr_store(tmp_path):
         sb.pp.pca(sb.read_zarr_backed(tmp_path / "x.zarr"), n_comps=5)
 
 
-def test_pca_overlapped_upload_equals_plain_upload(monkeypatch):
-    """`_ops.pca_csr` hides the host->device copy of large matrices behind the Gram accumulation (row ranges on a side
-    stream); the result must be the plain path's up to fp64 summation order.  Forced on a small matrix, incl. ranges that
-    fall on empty rows."""
-    from scanpy_b200 import _ops
-
-    x, _ = synth_scipy(9000, 500, n_clusters=6, r=40)
-    x = x.tolil()
-    x[3000:3400] = 0
-    x = x.tocsr().astype(np.float32)
-    x.eliminate_zeros()
-    monkeypatch.delenv("SB2_PCA_OVERLAP", raising=False)
-    plain = _ops.pca_csr(x, 25, solver=1)
-    monkeypatch.setenv("SB2_PCA_OVERLAP", "1")
-    monkeypatch.setenv("SB2_PCA_OVERLAP_MIN_NNZ", "1")
-    over = _ops.pca_csr(x, 25, solver=1)
-    scale = np.abs(plain["X_pca"]).max(axis=0)
-    assert (np.abs(plain["X_pca"] - over["X_pca"]) / scale).max() < 1e-6
-    np.testing.assert_allclose(over["components"], plain["components"], atol=1e-6)
-    np.testing.assert_allclose(over["variance"], plain["variance"], rtol=1e-10)
-    np.testing.assert_allclose(over["mean"], plain["mean"], rtol=1e-12, atol=1e-15)
-
-
 @pytest.mark.parametrize("solver", [None, "b200_spmm"])
 def test_pca_zero_center_false_matches_truncated_svd(solver):
     """`zero_center=False` = sklearn TruncatedSVD (src/scanpy/preprocessing/_pca/__init__.py:309-336): X V, V^T with
