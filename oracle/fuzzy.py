@@ -8,10 +8,13 @@ them from src/scanpy/neighbors/_connectivity.py:124-138:
     fuzzy_simplicial_set(coo((n,1)), n_neighbors, None, None, knn_indices=..., knn_dists=...,
                          set_op_mix_ratio=1.0, local_connectivity=1.0)  ->  .tocsr()
 
-Numerics follow umap's numba code: knn_dists are cast to float32; the sigma bisection runs
+Numerics follow umap's numba code: knn_dists are cast to float32; rho for a fractional
+local_connectivity is formed in float64 and rounded once; the sigma bisection runs
 in float64 scalars (numba types the Python floats lo/mid/hi as float64) and stores float32;
-membership strengths are float32.  The row loop is vectorised over rows with numpy (each
-row's bisection is independent; rows that hit the tolerance are frozen, as `break` does).
+membership strengths are float32.  The means of the sigma floor are summed in float64 (numba sums
+`np.mean` of a float32 array in float32, so a floored sigma can differ from umap's by a few float32
+ulps).  The row loop is vectorised over rows with numpy (each row's bisection is independent; rows
+that hit the tolerance are frozen, as `break` does).
 
 Pinned against: tests/test_neighbors.py:43-48 (`connectivities_umap`, 4 points) and the in-tree
 pbmc68k fixture (obsp/distances -> obsp/connectivities), see tests/test_oracle_goldens.py.
@@ -27,16 +30,22 @@ MIN_K_DIST_SCALE = 1e-3
 
 def smooth_knn_dist(distances: np.ndarray, k: float, *, n_iter: int = 64,
                     local_connectivity: float = 1.0, bandwidth: float = 1.0):
-    """-> (sigmas float32[n], rhos float32[n]).  distances: float32 [n, K], ascending rows."""
+    """-> (sigmas float32[n], rhos float32[n], margin float64[n]).  distances: float32 [n, K], rows in any order.
+
+    margin[i] is the smallest distance of row i's bisection from one of its decisions: the minimum over the
+    iterations run of |psum - target| (the `psum > target` branch) and of ||psum - target| - 1e-5| (the stopping
+    test).  An implementation whose psum differs by less than that takes every decision the same way, so it ends
+    on the same mid, bit for bit."""
     distances = np.asarray(distances, np.float32)
     n, K = distances.shape
     target = np.log2(k) * bandwidth
     rho = np.zeros(n, np.float32)
     mean_distances = float(np.mean(distances.astype(np.float64)))
 
-    # rho: umap_.py smooth_knn_dist, the `non_zero_dists` block
+    # rho: umap_.py smooth_knn_dist, the `non_zero_dists` block.  numba types `interpolation` as float64 and the
+    # difference of two float32 distances as float32; the product and sum are float64, rounded once into rho[i]
     index = int(np.floor(local_connectivity))
-    interpolation = local_connectivity - index
+    interpolation = float(local_connectivity) - index
     nzmask = distances > 0.0
     nnz = nzmask.sum(axis=1)
     # position (within the row) of the m-th non-zero entry, m = 0..: use a stable argsort of ~mask
@@ -47,9 +56,9 @@ def smooth_knn_dist(distances: np.ndarray, k: float, *, n_iter: int = 64,
         r = nz_sorted[:, index - 1].copy()
         if interpolation > SMOOTH_K_TOLERANCE:
             nxt = nz_sorted[:, min(index, K - 1)]
-            r = r + np.float32(interpolation) * (nxt - r)
+            r = (r.astype(np.float64) + interpolation * (nxt - r).astype(np.float64)).astype(np.float32)
     else:
-        r = np.float32(interpolation) * nz_sorted[:, 0]
+        r = (interpolation * nz_sorted[:, 0].astype(np.float64)).astype(np.float32)
     rho[enough] = r[enough]
     some = (~enough) & (nnz > 0)
     if some.any():
@@ -59,6 +68,7 @@ def smooth_knn_dist(distances: np.ndarray, k: float, *, n_iter: int = 64,
     hi = np.full(n, np.inf, np.float64)
     mid = np.ones(n, np.float64)
     active = np.ones(n, bool)
+    margin = np.full(n, np.inf)
     d = distances[:, 1:].astype(np.float32) - rho[:, None]  # float32 subtraction as in numba
     d64 = d.astype(np.float64)
     pos = d > 0
@@ -69,7 +79,9 @@ def smooth_knn_dist(distances: np.ndarray, k: float, *, n_iter: int = 64,
         with np.errstate(over="ignore", invalid="ignore", divide="ignore"):
             e = np.where(pos[a], np.exp(-(d64[a] / mid[a, None])), 1.0)
         psum = e.sum(axis=1)
-        done = np.abs(psum - target) < SMOOTH_K_TOLERANCE
+        gap = np.abs(psum - target)
+        margin[a] = np.minimum(margin[a], np.minimum(gap, np.abs(gap - SMOOTH_K_TOLERANCE)))
+        done = gap < SMOOTH_K_TOLERANCE
         ia = np.flatnonzero(a)
         active[ia[done]] = False
         ia, psum = ia[~done], psum[~done]
@@ -91,7 +103,7 @@ def smooth_knn_dist(distances: np.ndarray, k: float, *, n_iter: int = 64,
     floor = np.where(rho > 0.0, MIN_K_DIST_SCALE * mean_ith, MIN_K_DIST_SCALE * mean_distances)
     low = result < floor
     result[low] = floor[low].astype(np.float32)
-    return result, rho
+    return result, rho, margin
 
 
 def compute_membership_strengths(knn_indices, knn_dists, sigmas, rhos):
@@ -113,7 +125,7 @@ def fuzzy_simplicial_set(knn_indices, knn_dists, n_obs: int, n_neighbors: int, *
                          set_op_mix_ratio: float = 1.0, local_connectivity: float = 1.0):
     """-> scipy CSR float32, symmetric, zeros eliminated (what `umap()` returns at _connectivity.py:138)."""
     knn_dists = np.asarray(knn_dists).astype(np.float32)
-    sigmas, rhos = smooth_knn_dist(knn_dists, float(n_neighbors), local_connectivity=float(local_connectivity))
+    sigmas, rhos, _ = smooth_knn_dist(knn_dists, float(n_neighbors), local_connectivity=float(local_connectivity))
     rows, cols, vals = compute_membership_strengths(knn_indices, knn_dists, sigmas, rhos)
     result = sparse.coo_matrix((vals, (rows, cols)), shape=(n_obs, n_obs))
     result.eliminate_zeros()

@@ -306,9 +306,11 @@ def knn(x: np.ndarray, n_neighbors: int, *, ctx=None):
 
 # ------------------------------------------------------------------------------------------ graph
 def fuzzy_simplicial_set_device(ctx, d_idx, d_dist, n: int, k: int, *, set_op_mix_ratio: float = 1.0,
-                                local_connectivity: float = 1.0):
+                                local_connectivity: float = 1.0, self_first: bool = False):
+    """`self_first`: every list starts with its own cell (the kNN kernels' lists), whose weight is 0."""
     torch = _torch()
-    cap = 2 * n * max(k - 1, 1)
+    # every list entry adds at most one entry to its row and one to its neighbour's; a self column adds none
+    cap = 2 * n * (max(k - 1, 1) if self_first else k)
     indptr = torch.empty(n + 1, dtype=torch.int64, device="cuda")
     indices = torch.empty(cap, dtype=torch.int32, device="cuda")
     data = torch.empty(cap, dtype=torch.float32, device="cuda")
@@ -322,10 +324,23 @@ def fuzzy_simplicial_set_device(ctx, d_idx, d_dist, n: int, k: int, *, set_op_mi
     return indptr, indices[:m], data[:m], sig, rho
 
 
+def _refuse_repeated_ids(knn_indices: np.ndarray) -> None:
+    """The symmetrisation looks each edge's reverse up in the neighbour's list and takes the first match, while the
+    reference sums repeated (i, j) entries; so a k-list that names a neighbour twice is refused (-1 may repeat)."""
+    s = np.sort(np.asarray(knn_indices), axis=1)
+    rep = (s[:, 1:] == s[:, :-1]) & (s[:, 1:] >= 0)
+    if rep.any():
+        i = int(np.flatnonzero(rep.any(axis=1))[0])
+        j = int(s[i, 1:][rep[i]][0])
+        raise NotImplementedError(f"the k-list of row {i} names neighbour {j} more than once; repeated neighbour ids "
+                                  "are not implemented in scanpy_b200")
+
+
 def fuzzy_simplicial_set(knn_indices: np.ndarray, knn_dists: np.ndarray, *, ctx=None, **kw):
     """-> scipy CSR float32 connectivities (symmetric, sorted indices, no explicit zeros)."""
     from scipy import sparse
 
+    _refuse_repeated_ids(knn_indices)
     ctx = ctx or _abi.default_context()
     n, k = knn_indices.shape
     d_idx = _to_device(np.asarray(knn_indices, dtype=np.int32))
@@ -341,11 +356,12 @@ def knn_connectivities(knn_indices: np.ndarray, knn_dists: np.ndarray, method: s
     from scipy import sparse
 
     torch = _torch()
+    _refuse_repeated_ids(knn_indices)
     ctx = ctx or _abi.default_context()
     n, k = knn_indices.shape
     d_idx = _to_device(np.asarray(knn_indices, dtype=np.int32))
     d_dist = _to_device(np.asarray(knn_dists, dtype=np.float64))
-    cap = 2 * n * max(k - 1, 1)
+    cap = 2 * n * k
     indptr = torch.empty(n + 1, dtype=torch.int64, device="cuda")
     indices = torch.empty(cap, dtype=torch.int32, device="cuda")
     data = torch.empty(cap, dtype=torch.float64, device="cuda")
@@ -370,7 +386,7 @@ def knn_and_connectivities(x: np.ndarray, n_neighbors: int, *, ctx=None):
     if d_x is None or tuple(d_x.shape) != tuple(x.shape):
         d_x = _to_device(x)
     d_idx, d_dist, _ = knn_device(ctx, d_x, n_neighbors)
-    indptr, indices, data, _, _ = fuzzy_simplicial_set_device(ctx, d_idx, d_dist, n, n_neighbors)
+    indptr, indices, data, _, _ = fuzzy_simplicial_set_device(ctx, d_idx, d_dist, n, n_neighbors, self_first=True)
     # column 0 is the query itself by construction (knn_rescore_kernel / knn_fallback_kernel), cf. the reference's
     # `_get_sparse_matrix_from_indices_distances(..., keep_self=False)` (src/scanpy/neighbors/_common.py:35-61)
     nb_idx = d_idx[:, 1:].contiguous().view(-1)

@@ -141,7 +141,7 @@ __global__ void sym_count_kernel(int64_t n, int k, const int32_t* __restrict__ k
   const int32_t j = knn_idx[t];
   T c = (T)0;
   bool in_only = false;
-  if (j >= 0 && j != (int32_t)i) {
+  if (j >= 0) {  // a self entry (j == i) finds itself, so b = a: the fuzzy kernel's 0 stays 0, gauss / jaccard keep C[i,i]
     const T a = w[t];
     T b = (T)0;
     bool found = false;
@@ -221,7 +221,9 @@ sym_sort_rows_kernel(int64_t n, const int64_t* __restrict__ indptr, const int32_
 }
 
 // ---- method='jaccard' / 'gauss' directed weights (SURVEY 8f row f3), fp64 like the reference ----
-// jaccard (src/scanpy/neighbors/_connectivity.py:141-186): |N(i) & N(j)| / (2(k-1) - |N(i) & N(j)|), self excluded
+// jaccard (src/scanpy/neighbors/_connectivity.py:141-186): |N(i) & N(j)| / (2(k-1) - |N(i) & N(j)|), where N(i) is the
+// list without its column 0.  Column 0 is normally self; when it is not (a duplicate cell came first), self sits in
+// N(i) and gets J[i,i] = 1, as in the reference.
 __global__ void jaccard_rows_kernel(int64_t n, int k, const int32_t* __restrict__ knn_idx, double* __restrict__ w) {
   const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= n * k) return;
@@ -229,7 +231,7 @@ __global__ void jaccard_rows_kernel(int64_t n, int k, const int32_t* __restrict_
   const int m = (int)(t % k);
   const int32_t j = knn_idx[t];
   double val = 0.0;
-  if (m > 0 && j >= 0 && j != (int32_t)i) {
+  if (m > 0 && j >= 0) {
     const int32_t* li = knn_idx + i * k;
     const int32_t* lj = knn_idx + (int64_t)j * k;
     int shared = 0;
@@ -241,7 +243,8 @@ __global__ void jaccard_rows_kernel(int64_t n, int k, const int32_t* __restrict_
   }
   w[t] = val;
 }
-// gauss, sparse kNN branch (:17-100): sigma_i^2 = median of the k-1 squared neighbour distances
+// gauss, sparse kNN branch (:17-100): sigma_i^2 = median of the k-1 squared neighbour distances; every entry after
+// column 0 is weighted, self included when it is not first (its weight is exp(-d^2 / (2 sigma_i^2)))
 template <int MK>
 __global__ void gauss_sigma_kernel(int64_t n, int k, const double* __restrict__ knn_dist, double* __restrict__ sig_sq) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -265,7 +268,7 @@ __global__ void gauss_rows_kernel(int64_t n, int k, const int32_t* __restrict__ 
   const int m = (int)(t % k);
   const int32_t j = knn_idx[t];
   double val = 0.0;
-  if (m > 0 && j >= 0 && j != (int32_t)i) {
+  if (m > 0 && j >= 0) {
     const double si2 = sig_sq[i], sj2 = sig_sq[j];
     const double num = 2.0 * sqrt(si2) * sqrt(sj2), den = si2 + sj2;
     const double d = knn_dist[t];

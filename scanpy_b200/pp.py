@@ -187,8 +187,18 @@ def _get_sparse_matrix_from_indices_distances(indices, distances, *, keep_self: 
     return sparse.csr_matrix((data, cols, indptr), shape=(indices.shape[0],) * 2)
 
 
+def _short_row_error(i: int, stored: int, n_neighbors: int) -> ValueError:
+    return ValueError(f"row {i} of the distance matrix stores {stored} neighbour distances, fewer than the "
+                      f"n_neighbors - 1 = {n_neighbors - 1} that n_neighbors={n_neighbors} needs")
+
+
 def _get_indices_distances_from_sparse_matrix(d, n_neighbors: int):
-    """src/scanpy/neighbors/_common.py:74-143 (constant-nnz shortcut + slow path)."""
+    """src/scanpy/neighbors/_common.py:74-143 (constant-nnz shortcut + slow path).
+
+    Every row must give n_neighbors - 1 neighbours besides the cell itself; a shorter row raises `ValueError`.  The
+    reference's slow path raises there too (its `indices[i, 1:] = neighbors[1]` cannot broadcast), except for a
+    one-entry row, which it repeats; and its shortcut hands shorter lists to the kernels with the target log2(n_neighbors)
+    of the full width.  Padding would invent edges (to cell 0), so both are refused here."""
     nnzs = d.getnnz(axis=1)
     if len(nnzs) and (nnzs == nnzs[0]).all():
         n_obs, k = d.shape[0], int(nnzs[0])
@@ -197,6 +207,9 @@ def _get_indices_distances_from_sparse_matrix(d, n_neighbors: int):
         warn("Sparse matrix has no constant number of neighbors per row. Cannot efficiently get indices and "
              "distances.", RuntimeWarning)
         n_obs = d.shape[0]
+        short = np.flatnonzero(nnzs < n_neighbors - 1)
+        if len(short):
+            raise _short_row_error(int(short[0]), int(nnzs[short[0]]), n_neighbors)
         indices = np.zeros((n_obs, n_neighbors), dtype=int)
         distances = np.zeros((n_obs, n_neighbors), dtype=d.dtype)
         for i in range(n_obs):
@@ -206,11 +219,13 @@ def _get_indices_distances_from_sparse_matrix(d, n_neighbors: int):
                 o = np.argsort(vals)[: n_neighbors - 1]
                 cols, vals = cols[o], vals[o]
             indices[i, 0], distances[i, 0] = i, 0
-            indices[i, 1:1 + len(cols)] = cols
-            distances[i, 1:1 + len(cols)] = vals
+            indices[i, 1:] = cols
+            distances[i, 1:] = vals
     if not _has_self_column(indices, distances):
         indices = np.hstack([np.arange(indices.shape[0])[:, None], indices])
         distances = np.hstack([np.zeros(distances.shape[0])[:, None], distances])
+    if indices.shape[1] < n_neighbors:
+        raise _short_row_error(0, indices.shape[1] - 1, n_neighbors)
     if indices.shape[1] > n_neighbors:
         indices, distances = indices[:, :n_neighbors], distances[:, :n_neighbors]
     return indices, distances
@@ -276,14 +291,27 @@ def _neighbors_from_distances(adata, n_neighbors, *, distances, method, metric, 
         warn(f"Parameter(s) ignored if `distances` is given: {ignored}", UserWarning)
     if callable(metric):
         raise TypeError("`metric` must be a string if `distances` is given.")
+    if not 2 <= n_neighbors <= 64:
+        # the connectivity kernels of csrc/graph.cu hold a k-list of at most 64 entries in registers
+        raise NotImplementedError(f"n_neighbors={n_neighbors!r} with `distances`: scanpy_b200 computes "
+                                  "connectivities for 2 <= n_neighbors <= 64")
     start = log_start("computing connectivities")
     adata = adata.copy() if copy else adata
     if sparse.issparse(distances):
         distances = distances.tocsr(copy=True)
         distances.setdiag(0)
         distances.eliminate_zeros()
+        if method == "gauss" and (distances.getnnz(axis=1) > n_neighbors - 1).any():
+            # the reference weights every stored entry of such a row, the gauss kernels only its k-list
+            raise NotImplementedError("method='gauss' with `distances` rows that store more than n_neighbors - 1 "
+                                      "distances is not implemented in scanpy_b200")
         knn_indices, knn_distances = _get_indices_distances_from_sparse_matrix(distances, n_neighbors)
     else:
+        if method == "gauss":
+            # the reference's dense branch takes sigma_i^2 = (largest k-list squared distance) / 4 and returns a dense
+            # matrix; the gauss kernels implement its sparse branch only
+            raise NotImplementedError("method='gauss' with dense `distances` is not implemented in scanpy_b200; "
+                                      "pass a CSR matrix with n_neighbors - 1 distances per row")
         distances = np.asarray(distances).copy()
         np.fill_diagonal(distances, 0)
         knn_indices, knn_distances = _get_indices_distances_from_dense_matrix(distances, n_neighbors)

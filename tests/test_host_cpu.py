@@ -52,7 +52,7 @@ def test_product_never_imports_oracle():
         assert "oracle/" not in cu.read_text().replace("// oracle", ""), cu
 
 
-def test_indices_distances_roundtrip_matches_reference_helpers():
+def test_indices_distances_roundtrip_and_ragged_rows():
     # src/scanpy/neighbors/_common.py:35-98 ; tests/test_neighbors_common.py:59-103
     rs = np.random.RandomState(0)
     n, k = 40, 6
@@ -71,11 +71,17 @@ def test_indices_distances_roundtrip_matches_reference_helpers():
     np.testing.assert_allclose(d3, dist)
     with pytest.raises(AssertionError, match="first neighbor"):
         pp._get_sparse_matrix_from_indices_distances(idx[:, 1:], dist[:, 1:], keep_self=False)
-    # ragged rows -> slow path + RuntimeWarning (src/scanpy/neighbors/_common.py:101-123,126-143)
-    rag = m.tolil(); rag[0, idx[0, 1]] = 0; rag = rag.tocsr(); rag.eliminate_zeros()
+    # ragged rows -> slow path + RuntimeWarning (src/scanpy/neighbors/_common.py:101-123,126-143): a longer row keeps
+    # its k - 1 nearest, a shorter row is refused (padding it would invent edges to cell 0)
+    far = next(j for j in range(n) if j != 0 and j not in idx[0])
+    rag = m.tolil(); rag[0, far] = 2.0; rag = rag.tocsr()
     with pytest.warns(RuntimeWarning, match="no constant number"):
         i4, d4 = pp._get_indices_distances_from_sparse_matrix(rag, k)
     assert i4.shape == (n, k) and (i4[:, 0] == np.arange(n)).all()
+    np.testing.assert_array_equal(np.sort(i4, axis=1), np.sort(idx, axis=1))
+    short = m.tolil(); short[0, idx[0, 1]] = 0; short = short.tocsr(); short.eliminate_zeros()
+    with pytest.warns(RuntimeWarning, match="no constant number"), pytest.raises(ValueError, match="row 0 "):
+        pp._get_indices_distances_from_sparse_matrix(short, k)
 
 
 def test_random_state_shim():
