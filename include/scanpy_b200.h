@@ -216,7 +216,8 @@ int32_t sb2_louvain_csr_f32(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, co
  * sb2_log1p_f32             <- np.log1p(x.data) [/ log(base)] (src/scanpy/preprocessing/_simple.py:359-380), in place
  * sb2_csr_col_sums_f32      <- stats.mean_var(expm1(x), axis=0) inside highly_variable_genes(flavor='seurat')
  *                              (src/scanpy/preprocessing/_highly_variable_genes.py:337-346): per-gene sum and sum of
- *                              squares (fp64) of expm1(x * log_scale) (apply_expm1 = 1) or of x */
+ *                              squares (fp64) of expm1(x * log_scale) (apply_expm1 = 1; the product is formed in fp64
+ *                              and rounded once to float32, as numpy's `x *= np.log(base)` on float32 data) or of x */
 int32_t sb2_csr_row_sums_f32(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, const int32_t* d_indices,
                              const float* d_data, const int32_t* d_skip_cols, float* d_out);
 int32_t sb2_csr_hiexpr_count_f32(sb2_ctx* ctx, int64_t n, int32_t g, const int64_t* d_indptr, const int32_t* d_indices,

@@ -103,11 +103,13 @@ def hvg_seurat_from_stats(mean, var, *, n_top_genes=None, min_disp=0.5, max_disp
     return df.drop(columns=["mean_bin"])
 
 
-def scale(x, *, zero_center=True, max_value=None, mask_obs=None):
+def scale(x, *, zero_center=True, max_value=None, mask_obs=None, stats=None):
     """`scale_array` / `scale_array_masked` / `clip_array` / `scale_and_clip_csr`
     (src/scanpy/preprocessing/_scale.py:52-69,150-283) restated in numpy -> (x_scaled, mean, std).
     Pinned by the reference's goldens in tests/test_scaling.py:15-53 (X_original / X_scaled_original /
-    X_centered_original and their clipped / masked variants, reproduced in tests/golden/)."""
+    X_centered_original and their clipped / masked variants, reproduced in tests/golden/).
+    `stats=(mean, std)` skips the statistics and applies the arithmetic with the given float64 mean and std (a zero std
+    is used as given), so the scaling step can be compared on its own."""
     sp = sparse.issparse(x)
     if sp:
         x = sparse.csr_matrix(x).copy()
@@ -118,16 +120,19 @@ def scale(x, *, zero_center=True, max_value=None, mask_obs=None):
     sel = slice(None) if mask_obs is None else np.asarray(mask_obs, bool)
     sub = x[sel, :]
     n = sub.shape[0]
-    if sp:
-        d64 = sub.astype(np.float64)
-        mean = np.asarray(d64.mean(axis=0)).ravel()
-        mean_sq = np.asarray(d64.multiply(d64).mean(axis=0)).ravel()
+    if stats is not None:
+        mean, std = (np.asarray(s, np.float64) for s in stats)
     else:
-        mean = sub.mean(axis=0, dtype=np.float64)
-        mean_sq = np.multiply(sub, sub, dtype=np.float64).mean(axis=0, dtype=np.float64)
-    var = (mean_sq - mean**2) * (n / (n - 1))
-    std = np.sqrt(var)
-    std[std == 0] = 1
+        if sp:
+            d64 = sub.astype(np.float64)
+            mean = np.asarray(d64.mean(axis=0)).ravel()
+            mean_sq = np.asarray(d64.multiply(d64).mean(axis=0)).ravel()
+        else:
+            mean = sub.mean(axis=0, dtype=np.float64)
+            mean_sq = np.multiply(sub, sub, dtype=np.float64).mean(axis=0, dtype=np.float64)
+        var = (mean_sq - mean**2) * (n / (n - 1))
+        std = np.sqrt(var)
+        std[std == 0] = 1
     if sp and not zero_center:
         rows = np.repeat(np.arange(x.shape[0]), np.diff(x.indptr))
         on = np.ones(x.nnz, bool) if mask_obs is None else np.asarray(mask_obs, bool)[rows]
@@ -138,7 +143,7 @@ def scale(x, *, zero_center=True, max_value=None, mask_obs=None):
         return x, mean, std
     if sp:
         assert mask_obs is None
-        out = np.asarray(x.astype(np.float64).todense()) - mean  # `x -= mean` on a sparse matrix -> float64 dense
+        out = np.asarray(x.todense()) - mean  # `x -= mean` on a sparse matrix: todense (in x.dtype), then float64
         out = out / std
     else:
         out = sub.copy()

@@ -199,7 +199,13 @@ def _scale_array(x, *, zero_center: bool, max_value, mask_obs):
     is_sparse = sparse.issparse(x)
     if is_sparse:
         xs = _as_csr32(x)
-        d_indptr, d_indices, d_data = _ops.csr_to_device(xs)
+        # the reference's statistics (`x.multiply(x)`) and densification sum duplicate entries first; the kernels see one
+        # value per (row, column).  The uncentred output below keeps x's own entries, each divided and clipped.
+        xc = xs
+        if not xs.has_canonical_format:
+            xc = xs.copy()
+            xc.sum_duplicates()
+        d_indptr, d_indices, d_data = _ops.csr_to_device(xc)
         check(ctx.lib.sb2_csr_col_stats_rows_f32(ctx.handle, n, g, ptr(d_indptr), ptr(d_indices), ptr(d_data),
                                                  ptr(d_mask) if d_mask is not None else None, ptr(s1), ptr(s2)))
     else:
@@ -218,6 +224,8 @@ def _scale_array(x, *, zero_center: bool, max_value, mask_obs):
     std = torch.sqrt(var)
     std[std == 0] = 1
     if is_sparse and not zero_center:
+        if xc is not xs:
+            d_indptr, d_indices, d_data = _ops.csr_to_device(xs)
         check(ctx.lib.sb2_csr_scale_cols_f32(ctx.handle, n, ptr(d_indptr), ptr(d_indices), ptr(d_data), ptr(std),
                                              ptr(d_mask) if d_mask is not None else None, has_max, mx))
         out = sparse.csr_matrix((_ops._to_host(d_data), xs.indices, xs.indptr), shape=xs.shape)

@@ -53,16 +53,18 @@ __global__ void log1p_kernel(int64_t nnz, float* __restrict__ data, double log_b
   if (log_base != 0.0) v = (float)((double)v / log_base);  // np.divide(x, np.log(base)) (_simple.py:359-380)
   data[i] = v;
 }
-// per-gene sum and sum of squares of f(x), f = expm1(x * log_scale) (EXPM1) or identity; fp64 REDs into replicated copies
+// per-gene sum and sum of squares of f(x), f = expm1(x * log_scale) (EXPM1) or identity; fp64 REDs into replicated copies.
+// The product is taken in fp64 and rounded once to float32, as the reference's `x *= np.log(base)` on float32 data does
+// (a float32 multiply by the rounded log_scale is 1 ulp off for a few percent of x, which expm1 amplifies by ~x·ln b)
 constexpr int MV_COPIES = 32;
 template <bool EXPM1>
 __global__ void col_sums_transformed_kernel(int64_t nnz, const int32_t* __restrict__ indices, const float* __restrict__ data,
-                                            int g, double* __restrict__ acc, float log_scale) {
+                                            int g, double* __restrict__ acc, double log_scale) {
   double* mine = acc + (size_t)(blockIdx.x % MV_COPIES) * 2 * g;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nnz; i += (int64_t)gridDim.x * blockDim.x) {
     float x = data[i];
     if (EXPM1) {
-      if (log_scale != 1.0f) x *= log_scale;
+      if (log_scale != 1.0) x = (float)((double)x * log_scale);
       x = expm1f(x);
     }
     const double v = (double)x;
@@ -244,9 +246,9 @@ int32_t sb2_csr_col_sums_f32(sb2_ctx* ctx, int64_t nnz, int32_t g, const int32_t
   if (nnz > 0) {
     const unsigned grid = ctx->prop.multiProcessorCount * 8;
     if (apply_expm1)
-      col_sums_transformed_kernel<true><<<grid, 256, 0, ctx->stream>>>(nnz, d_indices, d_data, g, acc, (float)log_scale);
+      col_sums_transformed_kernel<true><<<grid, 256, 0, ctx->stream>>>(nnz, d_indices, d_data, g, acc, log_scale);
     else
-      col_sums_transformed_kernel<false><<<grid, 256, 0, ctx->stream>>>(nnz, d_indices, d_data, g, acc, (float)log_scale);
+      col_sums_transformed_kernel<false><<<grid, 256, 0, ctx->stream>>>(nnz, d_indices, d_data, g, acc, log_scale);
     SB2_LAUNCH_CHECK(ctx);
   }
   return finish_col_stats(ctx, acc, both, g, d_sum, d_sumsq);
