@@ -173,6 +173,14 @@ int32_t sb2_knn_l2_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, const float* d
 int32_t sb2_knn_debug_proposals_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, const float* d_x, int32_t terms,
                                     float* d_score, int32_t* d_idx, float* d_dnorm, double* h_meta);
 
+/* test / debug entry: the tile screen of a whole-data-set kNN call (k neighbours, d <= 150, fp16 tier), as the default
+ * sweep would use it at any size.  d_perm [n_points]: the kd order (position -> point; query block b holds the points
+ * at positions [128 b, 128 b + 128)); d_lists [blocks x tiles] / d_len [blocks]: per query block the ascending candidate
+ * tiles (of the order) it visits; d_ub [n_points]: per position the bound u >= the row's k-th neighbour distance that
+ * justified the skipped tiles (+inf: none). */
+int32_t sb2_knn_debug_screen_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, const float* d_x, int32_t k, int32_t* d_perm,
+                                 int32_t* d_lists, int32_t* d_len, float* d_ub);
+
 /* ---- UMAP fuzzy simplicial set -> symmetric connectivities CSR -------------------------------
  * d_knn_idx/d_knn_dist [n x k] (column 0 = self), as produced by sb2_knn_l2_f32; 2 <= k <= 64.
  * Output CSR: d_indptr int64[n+1], d_indices int32[cap], d_data float32[cap]; cap >= 2*n*(k-1) is

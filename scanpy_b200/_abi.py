@@ -85,6 +85,8 @@ SIGNATURES = {
                                  c_void_p, POINTER(KnnInfo)]),
     "sb2_knn_debug_proposals_f32": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p,
                                               c_void_p]),
+    "sb2_knn_debug_screen_f32": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_int32, c_void_p, c_void_p, c_void_p,
+                                           c_void_p]),
     "sb2_fuzzy_simplicial_set_f32": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_float, c_float,
                                                c_void_p, c_void_p, c_void_p, c_int64, POINTER(c_int64), c_void_p,
                                                c_void_p]),

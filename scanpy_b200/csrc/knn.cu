@@ -25,7 +25,9 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <type_traits>
+#include <vector>
 
 #include "common.cuh"
 #include "knn_internal.cuh"
@@ -240,7 +242,8 @@ __global__ void knn_rescore_kernel(const float* __restrict__ X, int64_t n_points
                                    int k, int sub, const float* __restrict__ cand_score, const int32_t* __restrict__ cand_idx,
                                    const unsigned int* __restrict__ maxnorm_bits, const float* __restrict__ inv_s2,
                                    double c_q, double c_n, const float* __restrict__ dnorm,
-                                   const unsigned int* __restrict__ dmax_bits, int32_t* __restrict__ idx_out,
+                                   const unsigned int* __restrict__ dmax_bits, const int32_t* __restrict__ cand_map,
+                                   const float* __restrict__ ubound, int32_t* __restrict__ idx_out,
                                    double* __restrict__ dist_out, int32_t* __restrict__ work_q,
                                    double* __restrict__ work_ub, unsigned long long* __restrict__ work_cnt) {
   constexpr int LM = 32 * R;
@@ -258,7 +261,8 @@ __global__ void knn_rescore_kernel(const float* __restrict__ X, int64_t n_points
   double qn = 0.0;
 #pragma unroll
   for (int r = 0; r < R; ++r) {
-    const int32_t ci = cand_idx[li * LM + r * 32 + lane];
+    int32_t ci = cand_idx[li * LM + r * 32 + lane];
+    if (cand_map && ci >= 0) ci = cand_map[ci];   // image position -> point
     cs[r] = cand_score[li * LM + r * 32 + lane];  // unused slots hold the sweep's starting threshold (-inf for a cold start)
     const float* xc = X + (int64_t)(ci < 0 ? 0 : ci) * d;
     double acc = 0.0, qq = 0.0;
@@ -359,6 +363,12 @@ __global__ void knn_rescore_kernel(const float* __restrict__ X, int64_t n_points
       if (!(r2s2 >= 9801.0 && r2s2 <= 67600.0)) certified = false;
     }
   }
+  // tile screen: the sweep skipped tiles with no point within ubound[li] of the row, so the row's k-th distance must be
+  // below it (with a margin far above the fp64 rounding of any squared distance)
+  if (ubound) {
+    const double u = (double)ubound[li];
+    certified = certified && kth <= u * u * (1.0 - 1e-9);
+  }
 #pragma unroll
   for (int r = 0; r < R; ++r) {
     const int e = r * 32 + lane;
@@ -371,6 +381,74 @@ __global__ void knn_rescore_kernel(const float* __restrict__ X, int64_t n_points
     const unsigned long long w = atomicAdd(work_cnt, 1ull);
     work_q[w] = (int32_t)ql;
     work_ub[w] = self_first ? kth : DBL_MAX;
+  }
+}
+
+
+// Tile screen, per launch row li (local row row_map[li]) after the short sweep of its block's own neighbourhood: at
+// least k proposals scored s_k or more, each with a true score >= s_k - eps (the fp16 tier's bound), so
+//   u^2 = |q|^2 - 2 (s_k - eps) >= d_k^2                                          -> ub[li] (rounded up)
+//   seed[li] = ((|q|^2 - u^2) / 2 - eps) / inv_s2: every point within u scores above it  (scaled units, rounded down)
+//   rowp[li] = (qlb, u s): qlb = (|q|^2 - 2 eps_c - slack) s^2, eps_c the bound for the centre image (exact fp16 centres:
+//              no |dc| term), slack 2^-19 (|q| + R)^2 s^2 covers the screen's fp32 arithmetic
+// Fewer than k proposals: u = +inf.  Rows n_rows <= li < n_pad (padding of the last block): rowp = (+inf, 0).
+template <int R>
+__global__ void knn_row_bound_kernel(const float* __restrict__ X, int d, int64_t q0, const int32_t* __restrict__ row_map, int64_t n_rows,
+                                     int64_t n_pad, int k, const float* __restrict__ cand_score, const int32_t* __restrict__ cand_idx,
+                                     const unsigned int* __restrict__ maxnorm_bits, const float* __restrict__ inv_s2, double c_q,
+                                     double c_n, const float* __restrict__ dnorm, const unsigned int* __restrict__ dmax_bits,
+                                     float* __restrict__ ub, float* __restrict__ seed, float2* __restrict__ rowp) {
+  constexpr int LM = 32 * R;
+  const int lane = threadIdx.x & 31;
+  const int64_t li = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (li >= n_pad) return;
+  if (li >= n_rows) {
+    if (lane == 0) rowp[li] = make_float2(INFINITY, 0.0f);
+    return;
+  }
+  const int64_t q = q0 + row_map[li];
+  double qq = 0.0;
+  for (int j = lane; j < d; j += 32) {
+    const double a = X[q * d + j];
+    qq = fma(a, a, qq);
+  }
+  const double qn = warp_sum(qq);
+  uint32_t kb[R];
+  int valid = 0;
+#pragma unroll
+  for (int r = 0; r < R; ++r) {
+    const bool ok = cand_idx[li * LM + r * 32 + lane] >= 0;
+    kb[r] = ok ? ord_bits(cand_score[li * LM + r * 32 + lane]) : 0u;
+    valid += ok;
+  }
+  valid = __reduce_add_sync(0xffffffffu, (unsigned)valid);
+  // the k-th largest proposal score: the largest t with #{kb >= t} >= k
+  uint32_t t = 0u;
+  for (int bit = 31; bit >= 0; --bit) {
+    const uint32_t cand = t | (1u << bit);
+    int c = 0;
+#pragma unroll
+    for (int r = 0; r < R; ++r) c += kb[r] >= cand;
+    if ((int)__reduce_add_sync(0xffffffffu, (unsigned)c) >= k) t = cand;
+  }
+  const double s2inv = (double)*inv_s2, s2 = 1.0 / s2inv;
+  const double Rn = sqrt((double)__uint_as_float(*maxnorm_bits)), qnorm = sqrt(qn);
+  const double dq = (double)dnorm[q], dc = (double)__uint_as_float(*dmax_bits);
+  const double eps_c = c_n * 0.5 * Rn * Rn + c_q * qnorm * Rn + dq * Rn * (1.0 + 1e-6);
+  const double eps = eps_c + (qnorm + dq) * dc * (1.0 + 1e-6);
+  const float sk = from_ord_bits(t);
+  float u = INFINITY, sd = -INFINITY;
+  if (valid >= k && isfinite(sk) && isfinite(qn)) {
+    const double u2 = qn - 2.0 * ((double)sk * s2inv - eps);
+    u = __double2float_ru(sqrt(fmax(u2, 0.0)) * (1.0 + 1e-7));
+    const double sdd = ((qn - (double)u * (double)u) * 0.5 - eps) * s2;
+    sd = __double2float_rd(sdd - fabs(sdd) * 1e-6);
+  }
+  if (lane == 0) {
+    ub[li] = u;
+    seed[li] = sd;
+    const double slack = 1.9073486328125e-06 * (qnorm + Rn) * (qnorm + Rn);   // 2^-19
+    rowp[li] = make_float2(__double2float_rd((qn - 2.0 * eps_c - slack) * s2), u * sqrtf((float)s2));
   }
 }
 
@@ -524,10 +602,12 @@ KnnSwitches knn_switches() {
     else s.cold = true;
   }
   if (const char* e = getenv("SB2_KNN_EST_RANK"); e && atoi(e) >= 1 && atoi(e) <= EST_R) s.est_rank = atoi(e);
-  if (const char* e = getenv("SB2_KNN_SCAN_SLOTS")) s.scan_slots = atoll(e);  // 0 forces the re-sweep (tests)
+  if (const char* e = getenv("SB2_KNN_SCAN_SLOTS")) s.scan_slots = atoll(e);
   s.pipe = !is("SB2_KNN_PIPE", "0");
   s.stamps = is("SB2_KNN_STAMPS", "1");
   s.int_scan = !is("SB2_KNN_SCAN", "float");
+  if (is("SB2_KNN_SCREEN", "0")) s.screen = 0;
+  else if (is("SB2_KNN_SCREEN", "1")) s.screen = 1;
   return s;
 }
 
@@ -579,15 +659,17 @@ struct Bound {
   int queue;
 };
 
-// fp64 re-score + certificate of n_rows proposal lists: launch row i is local row ql0 + i, or row_map[i] (ql0 = 0)
-int32_t launch_rescore(KnnCall& c, const Bound& b, int64_t ql0, const int32_t* row_map, int64_t n_rows) {
+// fp64 re-score + certificate of n_rows proposal lists (those of launch rows ql0 + i): launch row i is local row ql0 + i,
+// or row_map[i]; cand_map maps proposal ids (image positions) to points, ubound[i] is row i's tile-screen bound
+int32_t launch_rescore(KnnCall& c, const Bound& b, int64_t ql0, const int32_t* row_map, int64_t n_rows,
+                       const int32_t* cand_map = nullptr, const float* ubound = nullptr) {
   if (n_rows == 0) return SB2_OK;
   const int wpb = 8;
   const unsigned grid = (unsigned)ceil_div64(n_rows, wpb);
   const auto launch = [&](auto r) {
     knn_rescore_kernel<r><<<grid, wpb * 32, 0, c.ctx->stream>>>(
         c.d_x, c.n_points, c.d, c.q0, ql0, row_map, n_rows, c.k, c.sub, c.cand_score + ql0 * c.list_m,
-        c.cand_idx + ql0 * c.list_m, c.maxnorm, b.inv_s2, b.c_q, b.c_n, b.dnorm, b.dmax, c.d_idx, c.d_dist, c.wq[b.queue],
+        c.cand_idx + ql0 * c.list_m, c.maxnorm, b.inv_s2, b.c_q, b.c_n, b.dnorm, b.dmax, cand_map, ubound, c.d_idx, c.d_dist, c.wq[b.queue],
         c.wub[b.queue], c.wcnt + b.queue);
   };
   if (c.list_m == 32) launch(std::integral_constant<int, 1>());
@@ -605,21 +687,168 @@ int32_t read_count(sb2_ctx* ctx, const unsigned long long* d_cnt, int64_t* out) 
   return SB2_OK;
 }
 
+// The tile screen of tier 1 (knn_tc2.cu): both images in the kd order, and per 128-row query block the candidate tiles
+// that may hold a neighbour of one of its rows.  Launch row i (query image row i) is local row qloc[i].
+struct Screen {
+  int32_t* perm = nullptr;    // [n_points] image position -> point
+  int32_t* qloc = nullptr;    // [n_query]
+  int32_t* qpos = nullptr;    // [n_query] position of launch row i in perm (nullptr: i itself)
+  int32_t* lists = nullptr;   // block b's ascending tiles at lists[off[b] ..]; nullptr: every block sweeps every tile
+  int64_t* off = nullptr;     // [blocks]
+  int32_t* len = nullptr;     // [blocks]
+  std::vector<int32_t> h_len;
+  std::vector<int64_t> h_off;
+  float* ub = nullptr;        // [n_query] bound on the k-th neighbour distance
+  float* seed = nullptr;      // [n_query] starting threshold of the sweep (scaled score units)
+};
+
 // one precision tier of the tensor path (knn_tc2.cu): its sweep shape, its candidate image and its certificate
 struct Tier {
   KnnTc2Shape sh;
   __half* B = nullptr;
   Bound bound;
+  const Screen* scr = nullptr;   // tier 1 with the tile screen: B and the query image in the kd order
 };
 
-// one sweep of a tier, bracketed by the call's events, and the re-score of its proposals: local rows [ql0, ql0 + n_rows)
-// of the query image A, or (ql0 = 0) the rows row_map[0, n_rows) that A holds gathered in that order
-int32_t sweep_and_certify(KnnCall& c, const Tier& t, const __half* A, int64_t ql0, const int32_t* row_map, int64_t n_rows) {
+// one sweep of a tier, bracketed by the call's events, and the re-score of its proposals (launch rows [ql0, ql0 + n_rows)):
+// local rows [ql0, ql0 + n_rows) held by the query image A from its tile a_tile0 on, or the rows row_map[0, n_rows) that
+// A holds gathered in that order.  With the screen, row_map is the kd order's and each block walks its tile list.
+int32_t sweep_and_certify(KnnCall& c, const Tier& t, const __half* A, int64_t a_tile0, int64_t ql0, const int32_t* row_map,
+                          int64_t n_rows) {
+  KnnTc2Lists L{}, *lp = nullptr;
+  const bool lists = t.scr && t.scr->lists;   // without lists: the full sweep with the sampled estimate, in the kd order
+  if (t.scr) {
+    const Screen& S = *t.scr;
+    const int64_t b0 = ql0 / TILE, nb = ceil_div64(n_rows, TILE);
+    if (lists) {
+      int64_t total = 0;
+      for (int64_t b = b0; b < b0 + nb; ++b) total += S.h_len[b];
+      L = KnnTc2Lists{S.lists, 0, S.off + b0, S.len + b0, total, c.sw.cold ? nullptr : S.seed + ql0, c.sw.stamps};
+      lp = &L;
+    }
+    row_map = S.qloc + ql0;
+  }
   SB2_TRY(c.evs.begin());
-  SB2_TRY(knn_tc2_sweep(c.ctx, c.sw, t.sh, A, row_map ? 0 : (c.q0 + ql0) / TILE, t.B, c.n_points, n_rows, c.list_m,
-                        c.cand_score + ql0 * c.list_m, c.cand_idx + ql0 * c.list_m, &c.issued_flops));
+  SB2_TRY(knn_tc2_sweep(c.ctx, c.sw, t.sh, A, a_tile0, t.B, c.n_points, n_rows, c.list_m, c.cand_score + ql0 * c.list_m,
+                        c.cand_idx + ql0 * c.list_m, &c.issued_flops, lp));
   SB2_TRY(c.evs.end());
-  return launch_rescore(c, t.bound, ql0, row_map, n_rows);
+  return launch_rescore(c, t.bound, ql0, row_map, n_rows, t.scr ? t.scr->perm : nullptr, lists ? t.scr->ub + ql0 : nullptr);
+}
+
+// Above this share of kept (block, tile) pairs the screen's lists are dropped for the full sweep (SB2_KNN_SCREEN=1 keeps
+// them): see DESIGN.md §4 for the measurement behind it.
+constexpr double SCREEN_MAX_KEPT = 0.9;
+
+// Tier 1's images in the kd order and the tile screen: the order, the per-tile centres and radii, a short sweep of each
+// block's own neighbourhood (NEAR_TILES tiles) whose proposals bound every row's k-th distance (knn_row_bound_kernel),
+// then the screen of every row against every tile centre (knn_screen_kernel).  Bracketed by the call's events, so the
+// reported sweep time includes it; SB2_KNN_STAMPS=1 reports its parts.  The lists are kept (S.lists) when they skip
+// enough tiles (SCREEN_MAX_KEPT) and fit in device memory, or always with `force`; otherwise S.lists stays nullptr and
+// tier 1 sweeps every tile of the kd-ordered images from the sampled estimate, as without the screen.
+struct EventSet {   // CUDA events created on demand, destroyed on every exit
+  cudaEvent_t e[3] = {};
+  ~EventSet() {
+    for (cudaEvent_t x : e)
+      if (x) cudaEventDestroy(x);
+  }
+};
+int32_t screen_prep(KnnCall& c, Tier& t1, __half* A1, float* inv_s2, float* dnorm, bool force, Screen& S) {
+  sb2_ctx* ctx = c.ctx;
+  ScratchScope& scr = *c.scr;
+  cudaStream_t st = ctx->stream;
+  const int64_t n_points = c.n_points, n_query = c.n_query, n_tiles = ceil_div64(n_points, TILE);
+  const int64_t n_blocks = ceil_div64(n_query, TILE);
+  const int d = c.d;
+  EventSet evset;
+  cudaEvent_t* ev = evset.e;
+  if (c.sw.stamps)
+    for (int i = 0; i < 3; ++i) SB2_CUDA(cudaEventCreate(&ev[i]));
+  SB2_TRY(c.evs.begin());
+  if (ev[0]) SB2_CUDA(cudaEventRecord(ev[0], st));
+  SB2_TRY(scr.alloc(&S.perm, (size_t)n_points));
+  SB2_TRY(knn_tc2_kd_order(ctx, c.d_x, n_points, d, S.perm));
+  if (c.q0 == 0 && n_query == n_points) {
+    S.qloc = S.perm;
+  } else {
+    SB2_TRY(scr.alloc(&S.qloc, (size_t)n_query));
+    SB2_TRY(scr.alloc(&S.qpos, (size_t)n_query));
+    SB2_TRY(knn_tc2_restrict(ctx, S.perm, n_points, c.q0, n_query, S.qloc, S.qpos));
+  }
+  if (ev[1]) SB2_CUDA(cudaEventRecord(ev[1], st));
+  // images in the kd order (dnorm stays indexed by point)
+  SB2_TRY(knn_tc2_build_images(ctx, t1.sh, c.d_x, n_points, d, c.maxnorm, S.perm, 0, nullptr, t1.B, inv_s2, dnorm, c.maxnorm + 1));
+  SB2_TRY(knn_tc2_build_images(ctx, t1.sh, c.d_x, n_query, d, c.maxnorm, S.qloc, c.q0, A1, nullptr, inv_s2));
+  float *cent, *rad;
+  __half* Cimg;
+  SB2_TRY(scr.alloc(&cent, (size_t)n_tiles * d));
+  SB2_TRY(scr.alloc(&rad, (size_t)n_tiles));
+  SB2_TRY(scr.alloc(&Cimg, knn_tc2_b_halves(t1.sh, n_tiles)));
+  SB2_TRY(knn_tc2_tile_stats(ctx, c.d_x, n_points, d, S.perm, c.maxnorm, cent, rad));
+  SB2_TRY(knn_tc2_build_images(ctx, t1.sh, cent, n_tiles, d, c.maxnorm, nullptr, 0, nullptr, Cimg, inv_s2));
+  // the short sweep: cold, over each block's own neighbourhood
+  const int nt = knn_tc2_near_tiles();
+  int32_t *near, *near_len;
+  SB2_TRY(scr.alloc(&near, (size_t)n_blocks * nt));
+  SB2_TRY(scr.alloc(&near_len, (size_t)n_blocks));
+  SB2_TRY(knn_tc2_near_lists(ctx, n_blocks, n_tiles, S.qpos, near, near_len));
+  const KnnTc2Lists NL{near, nt, nullptr, near_len, n_blocks * (nt < n_tiles ? nt : n_tiles), nullptr, false};
+  SB2_TRY(knn_tc2_sweep(ctx, c.sw, t1.sh, A1, 0, t1.B, n_points, n_query, c.list_m, c.cand_score, c.cand_idx, &c.issued_flops, &NL));
+  float2* rowp;
+  SB2_TRY(scr.alloc(&S.ub, (size_t)n_query));
+  SB2_TRY(scr.alloc(&S.seed, (size_t)n_query));
+  SB2_TRY(scr.alloc(&rowp, (size_t)n_blocks * TILE));
+  {
+    const int wpb = 8;
+    const int64_t n_pad = n_blocks * TILE;
+    const unsigned grid = (unsigned)ceil_div64(n_pad, wpb);
+    const Bound& b = t1.bound;
+    const auto launch = [&](auto r) {
+      knn_row_bound_kernel<r><<<grid, wpb * 32, 0, st>>>(c.d_x, d, c.q0, S.qloc, n_query, n_pad, c.k, c.cand_score, c.cand_idx,
+                                                         c.maxnorm, inv_s2, b.c_q, b.c_n, dnorm, c.maxnorm + 1, S.ub, S.seed, rowp);
+    };
+    if (c.list_m == 64) launch(std::integral_constant<int, 2>());
+    else launch(std::integral_constant<int, 4>());
+    SB2_LAUNCH_CHECK(ctx);
+  }
+  // the screen writes a bitmap per block (n_tiles / 8 bytes) and its count; only the kept tiles become list entries
+  uint32_t* words;
+  SB2_TRY(scr.alloc(&words, (size_t)n_blocks * knn_tc2_screen_words(n_tiles)));
+  SB2_TRY(scr.alloc(&S.len, (size_t)n_blocks));
+  SB2_TRY(knn_tc2_screen(ctx, t1.sh, A1, Cimg, n_blocks, n_tiles, rowp, rad, c.maxnorm, words, S.len));
+  if (ev[2]) SB2_CUDA(cudaEventRecord(ev[2], st));
+  SB2_TRY(c.evs.end());
+  S.h_len.resize((size_t)n_blocks);
+  SB2_CUDA(cudaMemcpyAsync(S.h_len.data(), S.len, (size_t)n_blocks * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  SB2_CUDA(cudaStreamSynchronize(st));
+  S.h_off.resize((size_t)n_blocks);
+  int64_t total = 0;
+  for (int64_t b = 0; b < n_blocks; ++b) {
+    S.h_off[b] = total;
+    total += S.h_len[b];
+  }
+  const double kept = (double)total / ((double)n_blocks * (double)n_tiles);
+  size_t free_b = 0, total_b = 0;
+  SB2_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  const bool fits = (size_t)total * sizeof(int32_t) + (size_t)n_blocks * sizeof(int64_t) <= free_b / 4;
+  if (force || (kept <= SCREEN_MAX_KEPT && fits)) {
+    SB2_TRY(c.evs.begin());
+    SB2_TRY(scr.alloc(&S.off, (size_t)n_blocks));
+    SB2_TRY(scr.alloc(&S.lists, (size_t)total));
+    SB2_CUDA(cudaMemcpyAsync(S.off, S.h_off.data(), (size_t)n_blocks * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+    SB2_TRY(knn_tc2_expand_lists(ctx, words, n_blocks, n_tiles, S.off, S.lists));
+    SB2_TRY(c.evs.end());
+  }
+  if (ev[0]) {
+    float ms_order = 0.0f, ms_screen = 0.0f;
+    SB2_CUDA(cudaEventElapsedTime(&ms_order, ev[0], ev[1]));
+    SB2_CUDA(cudaEventElapsedTime(&ms_screen, ev[1], ev[2]));
+    std::vector<int32_t> v = S.h_len;
+    std::sort(v.begin(), v.end());
+    fprintf(stderr, "[sb2 knn screen] %lld blocks x %lld tiles: surviving %.4f, list length min %d median %d max %d; kd order %.2f ms, "
+            "images + short sweep + screen %.2f ms; %s\n", (long long)n_blocks, (long long)n_tiles, kept, v.front(), v[v.size() / 2],
+            v.back(), ms_order, ms_screen, S.lists ? "tile lists" : "full sweep (too few tiles skipped, or lists do not fit)");
+  }
+  return SB2_OK;
 }
 
 // Tensor path, in tiers that each end in the same fp64 re-score + certificate:
@@ -648,44 +877,71 @@ int32_t tensor_tiers(KnnCall& c) {
   t3.bound = {0.0, 0.0, inv_s2, nullptr, nullptr, 1};  // the split tier's for the exact scan
   knn_tc2_error_coefs(t1.sh, &t1.bound.c_q, &t1.bound.c_n);
   knn_tc2_error_coefs(t3.sh, &t3.bound.c_q, &t3.bound.c_n);
-  int64_t done = 0;  // local rows [0, done) have been through their first sweep
+  // the tile screen (SB2_KNN_SCREEN): by default from 512 candidate tiles on, below which the short sweep and the screen
+  // cost more than the tiles they can skip
+  const int64_t n_tiles = ceil_div64(n_points, TILE);
+  bool screen = !c.sw.split_only && t1.sh.nsplit == 1 && (c.sw.screen == 1 || (c.sw.screen < 0 && n_tiles >= 512));
+  if (screen) {   // the screen's bitmaps (n_q/128 x n/128 bits) must fit comfortably; otherwise the unscreened sweep
+    size_t free_b = 0, total_b = 0;
+    SB2_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    screen = (size_t)ceil_div64(n_query, TILE) * (size_t)knn_tc2_screen_words(n_tiles) * 4 <= free_b / 8;
+  }
+  Screen S;
+  int64_t done = 0;  // launch rows [0, done) have been through their first sweep
   if (!c.sw.split_only) {
     __half* A1;
     float* dnorm;  // |x - fp16(x)| per point; its maximum lives in maxnorm[1]
     SB2_TRY(scr.alloc(&A1, knn_tc2_a_halves(t1.sh, n_points)));
     SB2_TRY(scr.alloc(&t1.B, knn_tc2_b_halves(t1.sh, n_points)));
     SB2_TRY(scr.alloc(&dnorm, (size_t)n_points));
-    SB2_TRY(knn_tc2_build_images(ctx, t1.sh, c.d_x, n_points, d, c.maxnorm, nullptr, 0, A1, t1.B, inv_s2, dnorm, c.maxnorm + 1));
     t1.bound.dnorm = dnorm;
     t1.bound.dmax = c.maxnorm + 1;
-    // pilot: one wave of CTAs
+    if (screen) {
+      SB2_TRY(screen_prep(c, t1, A1, inv_s2, dnorm, c.sw.screen == 1, S));
+      t1.scr = &S;
+    } else {
+      SB2_TRY(knn_tc2_build_images(ctx, t1.sh, c.d_x, n_points, d, c.maxnorm, nullptr, 0, A1, t1.B, inv_s2, dnorm, c.maxnorm + 1));
+    }
+    const auto tile0 = [&](int64_t ql0) { return screen ? ql0 / TILE : (c.q0 + ql0) / TILE; };
+    // pilot: one wave of CTAs.  With the screen that wave is one contiguous region of the kd order, not a sample of the
+    // whole data set; what it decides (fp16 tier 1 for the rest, or split precision straight away) changes only the
+    // speed, every row is certified either way, and what makes the fp16 tier fail (the data's distance from the origin,
+    // relative to its neighbour gaps) is mostly a property of the whole embedding rather than of one region
     const int64_t wave = (int64_t)ctx->prop.multiProcessorCount * TILE;
     const int64_t first = n_query >= 4 * wave ? wave : n_query;
-    SB2_TRY(sweep_and_certify(c, t1, A1, 0, nullptr, first));
+    SB2_TRY(sweep_and_certify(c, t1, A1, tile0(0), 0, nullptr, first));
     done = first;
     if (first < n_query) {
       int64_t open1 = 0;
       SB2_TRY(read_count(ctx, c.wcnt, &open1));
       if (open1 * 2 <= first) {  // most pilot rows certified: tier 1 for the rest too
-        SB2_TRY(sweep_and_certify(c, t1, A1, done, nullptr, n_query - done));
+        SB2_TRY(sweep_and_certify(c, t1, A1, tile0(done), done, nullptr, n_query - done));
         done = n_query;
       }
     }
   }
   if (done < n_query) {
-    // split-precision sweep of the remaining rows, straight from the full image arrays
+    // split-precision sweep of the remaining rows, straight from the full image arrays (with the screen: the remaining
+    // launch rows, gathered, against the candidates in storage order)
     __half* A3;
     SB2_TRY(scr.alloc(&A3, knn_tc2_a_halves(t3.sh, n_points)));
     SB2_TRY(scr.alloc(&t3.B, knn_tc2_b_halves(t3.sh, n_points)));
-    SB2_TRY(knn_tc2_build_images(ctx, t3.sh, c.d_x, n_points, d, c.maxnorm, nullptr, 0, A3, t3.B, inv_s2));
-    SB2_TRY(sweep_and_certify(c, t3, A3, done, nullptr, n_query - done));
+    if (screen) {
+      SB2_TRY(knn_tc2_build_images(ctx, t3.sh, c.d_x, n_points, d, c.maxnorm, nullptr, 0, nullptr, t3.B, inv_s2));
+      SB2_TRY(knn_tc2_build_images(ctx, t3.sh, c.d_x, n_query - done, d, c.maxnorm, S.qloc + done, c.q0, A3, nullptr, inv_s2));
+      SB2_TRY(sweep_and_certify(c, t3, A3, 0, done, S.qloc + done, n_query - done));
+    } else {
+      SB2_TRY(knn_tc2_build_images(ctx, t3.sh, c.d_x, n_points, d, c.maxnorm, nullptr, 0, A3, t3.B, inv_s2));
+      SB2_TRY(sweep_and_certify(c, t3, A3, (c.q0 + done) / TILE, done, nullptr, n_query - done));
+    }
   }
   if (c.sw.split_only) return SB2_OK;
   // tier 2: gather the rows tier 1 left open and sweep them in split precision
   SB2_TRY(read_count(ctx, c.wcnt, &c.n_resweep));
-  // a re-sweep occupies one CTA per 128 open rows for a whole pass over the candidates (a few ms at 1.3M points
-  // however few rows there are); the exact scan streams the whole data set once per ROW (~45 us each at
-  // 1.3M x 50 once HBM saturates), so it only wins for a handful of rows
+  // a re-sweep occupies one CTA per 128 open rows for a whole pass over the candidates (9.4 ms at 1.3M x 50, however
+  // few rows there are); the exact scan gives each ROW one CTA that streams the whole data set, 21 ms for a single row
+  // at 1.3M x 50 (H100 80GB HBM3, 700 W): it only pays off as a bulk pass, so by default every open row is re-swept and
+  // the scan takes what the re-sweep leaves open (SB2_KNN_SCAN_SLOTS=n sends up to n rows straight to the scan)
   const int64_t n_resweep = c.n_resweep;
   if (n_resweep > 0 && n_resweep <= c.sw.scan_slots) {
     knn_append_queue_kernel<<<(unsigned)ceil_div64(n_resweep, 256), 256, 0, ctx->stream>>>(c.wq[0], c.wub[0], n_resweep, c.wq[1],
@@ -699,7 +955,7 @@ int32_t tensor_tiers(KnnCall& c) {
     __half* Ag;
     SB2_TRY(scr.alloc(&Ag, knn_tc2_a_halves(t3.sh, n_resweep)));
     SB2_TRY(knn_tc2_build_images(ctx, t3.sh, c.d_x, n_resweep, d, c.maxnorm, c.wq[0], c.q0, Ag, nullptr, inv_s2));
-    SB2_TRY(sweep_and_certify(c, t3, Ag, 0, c.wq[0], n_resweep));
+    SB2_TRY(sweep_and_certify(c, t3, Ag, 0, 0, c.wq[0], n_resweep));
   }
   return SB2_OK;
 }
@@ -785,6 +1041,45 @@ extern "C" int32_t sb2_knn_l2_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, con
     info->pass1_tensor = use_tc ? 2 : 0;
     info->n_resweep = c.n_resweep;
   }
+  return SB2_OK;
+}
+
+// Debug / test entry: the tile screen of a whole-data-set call (see include/scanpy_b200.h)
+extern "C" int32_t sb2_knn_debug_screen_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, const float* d_x, int32_t k, int32_t* d_perm,
+                                            int32_t* d_lists, int32_t* d_len, float* d_ub) {
+  SB2_CHECK_ARG(ctx && d_x && d_perm && d_lists && d_len && d_ub, "null pointer");
+  SB2_CHECK_ARG(n_points >= 1 && n_points < (int64_t)INT32_MAX - 2 * TILE && d >= 1 && d <= 150, "n_points / d");
+  SB2_CHECK_ARG(k >= 1 && k <= 56 && k <= n_points, "k must be in [1,56] and <= n_points");
+  const KnnSwitches sw = knn_switches();
+  SB2_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  ScratchScope scr(ctx);
+  KnnCall c{ctx, &scr, sw, d_x, n_points, 0, n_points, d, k, nullptr, nullptr};
+  SB2_TRY(prep_points(ctx, scr, d_x, n_points, d, &c.Xt, &c.maxnorm));
+  Tier t1;
+  SB2_CHECK_ARG(knn_tc2_shape(ctx, d, 1, true, &t1.sh) && t1.sh.nsplit == 1, "tile does not fit shared memory");
+  c.list_m = (k > 24 || sw.big_list) ? 128 : 64;
+  c.sub = c.list_m / 4;
+  SB2_TRY(scr.alloc(&c.cand_score, (size_t)n_points * c.list_m));
+  SB2_TRY(scr.alloc(&c.cand_idx, (size_t)n_points * c.list_m));
+  float *inv_s2, *dnorm;
+  __half* A1;
+  SB2_TRY(scr.alloc(&inv_s2, 4));
+  SB2_TRY(scr.alloc(&dnorm, (size_t)n_points));
+  SB2_TRY(scr.alloc(&A1, knn_tc2_a_halves(t1.sh, n_points)));
+  SB2_TRY(scr.alloc(&t1.B, knn_tc2_b_halves(t1.sh, n_points)));
+  t1.bound = {0.0, 0.0, inv_s2, dnorm, c.maxnorm + 1, 0};
+  knn_tc2_error_coefs(t1.sh, &t1.bound.c_q, &t1.bound.c_n);
+  Screen S;
+  SB2_TRY(screen_prep(c, t1, A1, inv_s2, dnorm, true, S));
+  const int64_t n_blocks = ceil_div64(n_points, TILE), n_tiles = ceil_div64(n_points, TILE);
+  SB2_CUDA(cudaMemcpyAsync(d_perm, S.perm, (size_t)n_points * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  for (int64_t b = 0; b < n_blocks; ++b)
+    SB2_CUDA(cudaMemcpyAsync(d_lists + b * n_tiles, S.lists + S.h_off[b], (size_t)S.h_len[b] * sizeof(int32_t),
+                             cudaMemcpyDeviceToDevice, st));
+  SB2_CUDA(cudaMemcpyAsync(d_len, S.len, (size_t)n_blocks * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  SB2_CUDA(cudaMemcpyAsync(d_ub, S.ub, (size_t)n_points * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  SB2_CUDA(cudaStreamSynchronize(st));
   return SB2_OK;
 }
 

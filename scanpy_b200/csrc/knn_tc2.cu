@@ -10,7 +10,7 @@
 // (d = 50: 64 and 160).  knn.cu runs terms = 1 first and re-sweeps the rows it cannot certify with terms = 3.
 //
 // Shape (one CTA per SM, 9 warps, or 12 in the pipelined loop):
-//   CTA = 128 queries x all candidate tiles of 128 points.
+//   CTA = 128 queries x the candidate tiles of 128 points on its list (all of them without the tile screen, below).
 //     warps 0-7   two consumer warpgroups; warpgroup g owns query rows 64g..64g+63 and issues, per tile, the k-steps of
 //                 wgmma.m64n128k16 (A = its 64 query rows, B = the staged candidate tile, both from shared memory, fp32
 //                 accumulators in registers) and examines the 64 x 128 scores in registers.  Pipelined loop (K = 64 and
@@ -25,14 +25,17 @@
 //     warp 8      producer: 1-D cp.async.bulk of pre-arranged candidate images (or K-slices of them) into an mbarrier
 //                 ring that takes the shared memory left after the query image (pipelined loop: warps 8-11, so that
 //                 setmaxnreg can hand their registers to the consumers)
-//   Starting threshold: the first n/16 visits sweep every 16th tile and keep the 6 largest chunk maxima per (row,
-//   sub-list); the four sub-lists of a row (four lanes of one warp) are merged by shuffles once and the 6th largest of
-//   the 24 seeds all four (rank ~96 of the row; SB2_KNN_EST_RANK picks another of the six).
-//   Sweep front: CTAs walk the candidate tiles cyclically, starting where the running CTAs currently are (g_knn2_front).
+//   Starting threshold: with the tile screen a per-row seed from its bound u(q); otherwise the first n/16 visits sweep
+//   every 16th tile and keep the 6 largest chunk maxima per (row, sub-list); the four sub-lists of a row (four lanes of
+//   one warp) are merged by shuffles once and the 6th largest of the 24 seeds all four (rank ~96 of the row;
+//   SB2_KNN_EST_RANK picks another of the six).
+//   Sweep front: CTAs walk their tile lists cyclically, starting where the running CTAs currently are (g_knn2_front).
 #include <cuda_fp16.h>
 #include <float.h>
 
 #include <type_traits>
+#include <utility>
+#include <vector>
 
 #include "common.cuh"
 #include "knn_internal.cuh"
@@ -76,8 +79,8 @@ __device__ __forceinline__ float tc_scale_from_maxnorm(unsigned int maxnorm_bits
 //   is_a = 1: A = [hi | hi | lo | 1 1 1]  (terms = 3)   or  [hi | 1 1 1]      (terms = 1)
 //   is_a = 0: B = [hi | lo | hi | h0 h1 h2]             or  [hi | h0 h1 h2]   with h0+h1+h2 = -|x|^2 s^2 / 2
 // gather != nullptr: image row r of tile t is point gather_base + gather[t*tile_rows + r]; rows past n are zero rows
-// (A) or score -60000 candidates (B).  dnorm[p] (optional) = |x_p - fp16(x_p)| in the units of X, rounded up;
-// *dmax_bits = its maximum (float bits).
+// (A) or score -60000 candidates (B).  dnorm[ps] (optional) = |x_ps - fp16(x_ps)| in the units of X, rounded up, indexed
+// by the point ps itself (not its image row); *dmax_bits = its maximum (float bits).
 __global__ void __launch_bounds__(256)
 knn_tc2_prep_kernel(const float* __restrict__ X, int64_t n, int d, int kpad, int terms, int tile_rows, int is_a,
                     const unsigned int* __restrict__ maxnorm_bits, const int32_t* __restrict__ gather, int64_t gather_base,
@@ -103,7 +106,7 @@ knn_tc2_prep_kernel(const float* __restrict__ X, int64_t n, int d, int kpad, int
       }
       if (dnorm) {
         const float dn = __double2float_ru(sqrt(dacc) * (1.0 + 1e-12) / (double)s);
-        dnorm[p] = dn;
+        dnorm[ps] = dn;
         atomicMax(dmax_bits, __float_as_uint(dn));
       }
       const double hn = -0.5 * acc;
@@ -267,14 +270,18 @@ __device__ __forceinline__ void est_chunk(float (&est)[LEN], const uint32_t (&v)
   est_push(est, chunk_max(v));
 }
 
-// nks = k-steps (16 columns of the K axis) per staged slice, nsplit = slices per candidate image.
-// Sweep front: CTAs walk the candidate tiles cyclically, each starting where the CTAs already running currently are
-// (the order of the candidates is irrelevant to the result).  All resident CTAs then stream the same few tiles at the
+// nks = k-steps (16 columns of the K axis) per staged slice, nsplit = slices per candidate image.  lists / list_len:
+// the ascending candidate tiles of each CTA, from lists[list_off[cta]] or lists[cta * list_stride] (list_stride = 0 and
+// list_len = nullptr: one list of all n_btiles tiles);
+// seed (optional): each launch row's starting threshold in place of the sampled estimate.
+// Sweep front: CTAs walk their lists cyclically, each starting at the first entry at or after the tile where the CTAs
+// already running currently are (the order of the candidates is irrelevant to the result).  All resident CTAs then stream the same few tiles at the
 // same time and the candidate images (166 MB at 1.3M x 50, more than the L2) are read from HBM about once per wave of
 // CTAs instead of once per CTA.  "Where the running CTAs are" is the MEAN position of the pack, (sweep visits so far) /
 // (resident CTAs): starting a new CTA at the position last published by ANY running CTA lets the spread of the pack
-// grow from wave to wave; re-centring every new CTA on the mean bounds it by the drift of a single lap.
-__device__ unsigned long long g_knn2_front;   // sweep-proper visits of all CTAs of this launch, in units of 16 tiles
+// grow from wave to wave; re-centring every new CTA on the mean bounds it by the drift of a single lap.  Progress is
+// counted in tiles advanced along the walk (not visits), so that CTAs with short lists keep pace in tile space.
+__device__ unsigned long long g_knn2_front;   // tiles the sweep-proper walks of all CTAs of this launch have advanced
 // PNKS = 0: single-buffer loop.  Per tile, a warpgroup issues its nks k-steps, waits for all of them, releases the stage
 //   and scans; the only overlap is whatever the other warpgroup's MMAs happen to do meanwhile.  Any nsplit / nstage.
 // PNKS > 0: pipelined loop, nks = PNKS.  Two accumulator sets; tile c+1's MMAs are issued (and run) while the warpgroup
@@ -293,7 +300,9 @@ template <int NG, int PNKS, bool STAMPS, bool ISCAN>
 __global__ void __launch_bounds__(PNKS > 0 ? THREADS_PIPE : THREADS, 1)
 knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bimg, int nks, int nsplit, int nstage,
                   int64_t n_btiles, int64_t n_est, int64_t est_stride, int est_rank, int64_t qtile0, int64_t n_query,
-                  int32_t n_points, float* __restrict__ cand_score, int32_t* __restrict__ cand_idx,
+                  int32_t n_points, const int32_t* __restrict__ lists, int64_t list_stride, const int64_t* __restrict__ list_off,
+                  const int32_t* __restrict__ list_len,
+                  const float* __restrict__ seed, float* __restrict__ cand_score, int32_t* __restrict__ cand_idx,
                   unsigned long long* __restrict__ stamps) {
   constexpr bool PIPE = PNKS > 0;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -305,11 +314,14 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
   uint64_t* full = bars;                  // [MAXST] producer -> consumers
   uint64_t* empty = bars + MAXST;         // [MAXST] consumer warps -> producer
   uint64_t* afull = bars + 2 * MAXST;     // [1]
-  int32_t* start_tile = reinterpret_cast<int32_t*>(bars + 2 * MAXST + 1);
+  int32_t* start_pos = reinterpret_cast<int32_t*>(bars + 2 * MAXST + 1);
   unsigned long long* stamp_sm = reinterpret_cast<unsigned long long*>(bars + 2 * MAXST + 2);  // [2][PH_N + 1]
   static_assert((2 * MAXST + 2 + 2 * (PH_N + 1)) * 8 <= BAR_BYTES, "barrier block");
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  // the candidate tiles this CTA visits after its estimate: lst[0, len), ascending
+  const int32_t* lst = lists + (list_off ? list_off[blockIdx.x] : (int64_t)blockIdx.x * list_stride);
+  const int32_t len = list_len ? list_len[blockIdx.x] : (int32_t)n_btiles;
   if (threadIdx.x == 0) {
     for (int s = 0; s < nstage; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], NCONS); }
     mbar_init(afull, 1);
@@ -318,8 +330,16 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
     unsigned int nsm;
     asm volatile("mov.u32 %0, %%nsmid;" : "=r"(nsm));
     const unsigned long long resident = min((unsigned long long)gridDim.x, (unsigned long long)max(nsm, 1u));
-    // mean tile of the pack now, plus the n_est visits this CTA spends on its threshold estimate before it joins
-    *start_tile = (int32_t)((f * 16ull / resident + (unsigned long long)n_est) % (unsigned long long)n_btiles);
+    // mean tile of the pack now, plus the n_est visits this CTA spends on its threshold estimate before it joins; the
+    // walk starts at the first list entry at or after it
+    const int32_t pos = (int32_t)((f / resident + (unsigned long long)n_est) % (unsigned long long)n_btiles);
+    int32_t lo = 0, hi = len;
+    while (lo < hi) {
+      const int32_t mid = (lo + hi) >> 1;
+      if (lst[mid] < pos) lo = mid + 1;
+      else hi = mid;
+    }
+    *start_pos = lo == len ? 0 : lo;
   }
   __syncthreads();
 
@@ -333,10 +353,10 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
       int s = 0;
       uint32_t use_phase = 1;  // parity of the previous use of stage s (first lap: nothing to wait for)
       bool first_lap = true;
-      int64_t cs = *start_tile;   // cyclic walk of the sweep proper
-      for (int64_t v = 0; v < n_est + n_btiles; ++v) {
+      int32_t cs = *start_pos;   // cyclic walk of the list
+      for (int64_t v = 0; v < n_est + len; ++v) {
         int64_t c = v * est_stride;
-        if (v >= n_est) { c = cs; if (++cs == n_btiles) cs = 0; }
+        if (v >= n_est) { c = lst[cs]; if (++cs == len) cs = 0; }
         for (int p = 0; p < nsplit; ++p) {
           if (!first_lap) mbar_wait(&empty[s], use_phase);
           mbar_expect_tx(&full[s], part_b);
@@ -380,10 +400,12 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
   const uint64_t db0 = wgmma_desc(smem_u32(Bs0), LBO, SBO);
   constexpr uint32_t KSTEP16 = (2u * LBO) >> 4;
   const uint32_t part16 = part_b >> 4;
-  const int n_visit = (int)(n_est + n_btiles), n_est_i = (int)n_est;
-  int32_t ctile = *start_tile;                 // candidate tile of the current sweep visit (cyclic walk)
+  const int n_visit = (int)(n_est + len), n_est_i = (int)n_est;
+  int32_t lpos = *start_pos;                   // list position of the current sweep visit (cyclic walk)
+  int32_t ctile = lst[lpos];                   // its candidate tile
   int32_t cbase = ctile * CN + 2 * sl;
   const int32_t n_bt = (int32_t)n_btiles;
+  uint32_t adv = 0;                            // warp 0 lane 0: tiles the walk advanced since the last front update
 
   // phase stamps (opt-in): no code at all without STAMPS
   const bool stamp_on = STAMPS && (warp & 3) == 0;
@@ -426,8 +448,9 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
         e0 = i < est_rank ? L0.ls[i] : e0;
         e1 = i < est_rank ? L1.ls[i] : e1;
       }
-      const float t0 = valid0 ? e0 : INFINITY;  // rows past n_query never accept anything
-      const float t1 = valid1 ? e1 : INFINITY;
+      // rows past n_query never accept anything; a per-row seed (from the tile screen's bound) replaces the estimate
+      const float t0 = valid0 ? (seed ? seed[ql0] : e0) : INFINITY;
+      const float t1 = valid1 ? (seed ? seed[ql1] : e1) : INFINITY;
 #pragma unroll
       for (int i = 0; i < LS; ++i) { L0.ls[i] = t0; L1.ls[i] = t1; }
 #pragma unroll
@@ -447,6 +470,8 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
       est_chunk(L0.ls, v0);
       est_chunk(L1.ls, v1);
     } else {
+      const int32_t npos = lpos + 1 == len ? 0 : lpos + 1;
+      const int32_t ntile = lst[npos];   // the next visit's tile, loaded under the scan
       bool hit0, hit1, redo = false;
       if constexpr (ISCAN) {
         const int t0 = __float_as_int(L0.tau), t1 = __float_as_int(L1.tau);
@@ -474,9 +499,13 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
         }
       }
       stamp(PH_INSERT);
-      if ((c & 15) == 0 && warp == 0 && lane == 0) atomicAdd(&g_knn2_front, 1ull);   // 16 more visits of the pack
-      cbase += CN;
-      if (++ctile == n_bt) { ctile = 0; cbase = 2 * sl; }
+      if (warp == 0 && lane == 0) {   // the pack's front, in tiles, published every 16 visits
+        adv += (uint32_t)(ntile > ctile ? ntile - ctile : ntile - ctile + n_bt);
+        if ((c & 15) == 0) { atomicAdd(&g_knn2_front, (unsigned long long)adv); adv = 0; }
+      }
+      lpos = npos;
+      ctile = ntile;
+      cbase = ntile * CN + 2 * sl;
     }
   };
 
@@ -589,6 +618,343 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
   }
 }
 
+
+// ------------------------------------------------------------------------------------------------
+// Tile-compact order and tile screen (SB2_KNN_SCREEN, on by default from 512 candidate tiles).
+//
+// kd order: the points are split recursively, each segment at a multiple of 128 points on the coordinate of largest
+// (sampled) variance, until every segment is one tile; knn.cu builds the fp16 images in that order, so each 128-point
+// candidate tile and each 128-row query block is spatially compact.  Per tile a centre mu_t and a radius r_t bound every
+// point of the tile: |q - x| >= |q - mu_t| - r_t.  The screen scores every query row against every centre on the tensor
+// cores (the centres go through the same image builder) and keeps, per query block, the tiles for which some row has
+// |q - mu_t| - r_t <= u(q), where u(q) >= d_k(q) comes from a short sweep of the block's own neighbourhood.  A skipped
+// tile holds no point within u(q) of any row of the block; the re-score checks d_k(q) <= u(q) before it certifies a row.
+constexpr int KD_SAMPLES = 512;   // points per segment the split coordinate is chosen from
+constexpr int KD_THREADS = 1024;
+constexpr int NEAR_TILES = 8;     // tiles of the short sweep that gives u(q): the block's own tile and its neighbours
+
+// segment s of a level = [seg[3s], seg[3s+2]), split at seg[3s+1]: its coordinate of largest variance over an evenly
+// spaced sample of its points (any choice is correct; the variance only makes the tiles tight)
+__global__ void __launch_bounds__(256) kd_axis_kernel(const float* __restrict__ X, int d, const int32_t* __restrict__ P,
+                                                      const int32_t* __restrict__ seg, int32_t* __restrict__ axis) {
+  __shared__ double var[256];
+  const int64_t a = seg[3 * blockIdx.x], len = seg[3 * blockIdx.x + 2] - a;
+  const int64_t ns = min(len, (int64_t)KD_SAMPLES);
+  const int j = threadIdx.x;
+  if (j < d) {
+    double s = 0.0, s2 = 0.0;
+    for (int64_t t = 0; t < ns; ++t) {
+      const double v = X[(int64_t)P[a + t * len / ns] * d + j];
+      s += v;
+      s2 += v * v;
+    }
+    var[j] = s2 - s * s / (double)ns;
+  }
+  __syncthreads();
+  if (j == 0) {
+    int best = 0;
+    for (int i = 1; i < d; ++i)
+      if (var[i] > var[best]) best = i;
+    axis[blockIdx.x] = best;
+  }
+}
+
+__global__ void kd_keys_kernel(const float* __restrict__ X, int d, const int32_t* __restrict__ P, const int32_t* __restrict__ seg,
+                               const int32_t* __restrict__ axis, uint32_t* __restrict__ key) {
+  const int64_t a = seg[3 * blockIdx.x], b = seg[3 * blockIdx.x + 2];
+  const int ax = axis[blockIdx.x];
+  for (int64_t i = a + (int64_t)blockIdx.y * blockDim.x + threadIdx.x; i < b; i += (int64_t)gridDim.y * blockDim.x)
+    key[i] = ord_bits(X[(int64_t)P[i] * d + ax]);
+}
+
+// inclusive prefix sum of one value per thread over the CTA (in thread order); *total = the sum
+__device__ __forceinline__ int block_scan_incl(int v, int* wsum, int* total) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int t = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += t;
+  }
+  if (lane == 31) wsum[w] = v;
+  __syncthreads();
+  if (w == 0) {
+    int s = lane < nw ? wsum[lane] : 0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, s, o);
+      if (lane >= o) s += t;
+    }
+    wsum[lane] = s;
+  }
+  __syncthreads();
+  const int r = v + (w > 0 ? wsum[w - 1] : 0);
+  *total = wsum[nw - 1];
+  __syncthreads();
+  return r;
+}
+
+// one CTA per segment: the m - a smallest keys (equal keys in position order) go to [a, m), the rest to [m, b), both
+// in position order.  The pivot is found by a 4-pass radix select over the 32-bit keys (histogram counts aggregated per
+// warp: the top byte of nearby floats is nearly constant); the partition takes KD_PER consecutive keys per thread.
+constexpr int KD_PER = 4;
+__global__ void __launch_bounds__(KD_THREADS) kd_split_kernel(const int32_t* __restrict__ seg, const uint32_t* __restrict__ key,
+                                                              const int32_t* __restrict__ P, int32_t* __restrict__ Pout) {
+  __shared__ unsigned hist[256];
+  __shared__ uint32_t s_prefix;
+  __shared__ int s_rank;
+  __shared__ int wsum[32];
+  const int64_t a = seg[3 * blockIdx.x], m = seg[3 * blockIdx.x + 1], b = seg[3 * blockIdx.x + 2];
+  const int lane = threadIdx.x & 31;
+  uint32_t prefix = 0;
+  int rank = (int)(m - a) - 1;   // sorted index of the pivot
+  for (int byte = 3; byte >= 0; --byte) {
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0u;
+    __syncthreads();
+    const uint32_t hmask = byte == 3 ? 0u : (0xffffffffu << (8 * (byte + 1)));
+    for (int64_t base = a; base < b; base += blockDim.x) {
+      const int64_t i = base + threadIdx.x;
+      const uint32_t k = i < b ? key[i] : 0u;
+      const unsigned bin = (i < b && (k & hmask) == prefix) ? (k >> (8 * byte)) & 255u : 256u;
+      const unsigned peers = __match_any_sync(0xffffffffu, bin);
+      if (bin < 256u && lane == __ffs(peers) - 1) atomicAdd(&hist[bin], (unsigned)__popc(peers));
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int r = rank, bin = 0;
+      for (; bin < 255; ++bin) {
+        if (r < (int)hist[bin]) break;
+        r -= (int)hist[bin];
+      }
+      s_prefix = prefix | ((uint32_t)bin << (8 * byte));
+      s_rank = r;
+    }
+    __syncthreads();
+    prefix = s_prefix;
+    rank = s_rank;
+    __syncthreads();
+  }
+  const uint32_t pivot = prefix;
+  const int eq_take = rank + 1;   // keys equal to the pivot that go left, the first ones in position order
+  int eq_before = 0, left_before = 0;
+  for (int64_t base = a; base < b; base += (int64_t)blockDim.x * KD_PER) {
+    const int64_t i0 = base + (int64_t)threadIdx.x * KD_PER;
+    uint32_t k[KD_PER];
+    int e_cnt = 0;
+#pragma unroll
+    for (int j = 0; j < KD_PER; ++j) {
+      k[j] = i0 + j < b ? key[i0 + j] : 0u;
+      e_cnt += i0 + j < b && k[j] == pivot;
+    }
+    int tot;
+    int eq_rank = eq_before + block_scan_incl(e_cnt, wsum, &tot) - e_cnt;
+    eq_before += tot;
+    unsigned lf = 0u;
+#pragma unroll
+    for (int j = 0; j < KD_PER; ++j) {
+      const bool in = i0 + j < b, e = in && k[j] == pivot;
+      lf |= (unsigned)(in && (k[j] < pivot || (e && eq_rank < eq_take))) << j;
+      eq_rank += e;
+    }
+    const int l_cnt = __popc(lf);
+    int64_t left_ex = left_before + block_scan_incl(l_cnt, wsum, &tot) - l_cnt;
+    left_before += tot;
+#pragma unroll
+    for (int j = 0; j < KD_PER; ++j) {
+      const int64_t i = i0 + j;
+      if (i < b) {
+        const bool l = (lf >> j) & 1u;
+        Pout[l ? a + left_ex : m + (i - a - left_ex)] = P[i];
+        left_ex += l;
+      }
+    }
+  }
+}
+
+__global__ void kd_iota_kernel(int32_t* __restrict__ P, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) P[i] = (int32_t)i;
+}
+
+// the call's query rows [q0, q0 + nq) in the order P puts them: qloc[j] = local row, qpos[j] = its position in P
+__global__ void __launch_bounds__(KD_THREADS) kd_restrict_kernel(const int32_t* __restrict__ P, int64_t n, int64_t q0, int64_t nq,
+                                                                 int32_t* __restrict__ qloc, int32_t* __restrict__ qpos) {
+  __shared__ int wsum[32];
+  int before = 0;
+  for (int64_t base = 0; base < n; base += blockDim.x) {
+    const int64_t i = base + threadIdx.x;
+    const int64_t ql = i < n ? (int64_t)P[i] - q0 : -1;
+    const int f = ql >= 0 && ql < nq;
+    int tot;
+    const int incl = block_scan_incl(f, wsum, &tot);
+    if (f) {
+      qloc[before + incl - 1] = (int32_t)ql;
+      qpos[before + incl - 1] = (int32_t)i;
+    }
+    before += tot;
+  }
+}
+
+// per tile t of the order P: the centre mu_t (the tile mean, rounded so that s * mu_t is an fp16 number, which the
+// candidate image then holds exactly) and rad[t] >= max |x - mu_t| over the tile's points (fp64, rounded up)
+__global__ void __launch_bounds__(256) kd_tile_stats_kernel(const float* __restrict__ X, int64_t n, int d, const int32_t* __restrict__ P,
+                                                            const unsigned int* __restrict__ maxnorm_bits, float* __restrict__ cent,
+                                                            float* __restrict__ rad) {
+  __shared__ float mu[256];
+  __shared__ unsigned int rmax;
+  const int64_t t = blockIdx.x, p0 = t * CN;
+  const int rows = (int)min((int64_t)CN, n - p0);
+  const float s = tc_scale_from_maxnorm(*maxnorm_bits);
+  if (threadIdx.x == 0) rmax = 0u;
+  if ((int)threadIdx.x < d) {
+    double acc = 0.0;
+    for (int r = 0; r < rows; ++r) acc += X[(int64_t)P[p0 + r] * d + threadIdx.x];
+    const float m = __half2float(__float2half_rn((float)(acc / rows) * s)) / s;
+    mu[threadIdx.x] = m;
+    cent[t * d + threadIdx.x] = m;
+  }
+  __syncthreads();
+  if ((int)threadIdx.x < rows) {
+    const float* x = X + (int64_t)P[p0 + threadIdx.x] * d;
+    double acc = 0.0;
+    for (int j = 0; j < d; ++j) {
+      const double df = (double)x[j] - (double)mu[j];
+      acc = fma(df, df, acc);
+    }
+    atomicMax(&rmax, __float_as_uint(__double2float_ru(sqrt(acc) * (1.0 + 1e-12))));
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) rad[t] = __uint_as_float(rmax);
+}
+
+// the short sweep's lists: NEAR_TILES consecutive tiles of the order around the tile of the block's first row
+__global__ void knn_near_lists_kernel(int64_t n_blocks, int64_t n_tiles, const int32_t* __restrict__ qpos, int32_t* __restrict__ lists,
+                                      int32_t* __restrict__ len) {
+  const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= n_blocks) return;
+  const int64_t own = (qpos ? (int64_t)qpos[b * QM] : b * QM) / CN;
+  const int64_t cnt = min((int64_t)NEAR_TILES, n_tiles);
+  const int64_t first = max((int64_t)0, min(own - NEAR_TILES / 2 + 1, n_tiles - cnt));
+  for (int64_t i = 0; i < cnt; ++i) lists[b * NEAR_TILES + i] = (int32_t)(first + i);
+  len[b] = (int32_t)cnt;
+}
+
+// The screen: CTA = one 128-row query block, two warpgroups score it against 128 tile centres at a time (wgmma from
+// shared memory, plain loads: the centre image is small and stays in L2).  rowp[row] = (qlb, us) in the images' scaled
+// units: qlb <= |q|^2 - 2 eps_c - (fp32 slack), so |q - mu|^2 >= qlb - 2 score for the computed score; us >= u(q)
+// (qlb = +inf: a padding row, which keeps nothing; us = +inf keeps everything).  Tile t survives if some row has
+// qlb - 2 score <= (us + s r_t)^2 (1 + 2^-16), tested as !(>) so that a NaN keeps it.  Output: the surviving tiles of
+// the block as a bitmap (bit t of words[block * n_words + t / 32]) and their count; knn_expand_lists_kernel turns the
+// bitmaps into compact lists once the counts are known, so the lists take 4 B per kept (block, tile) pair.
+__global__ void __launch_bounds__(256) knn_screen_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Cimg, int nks,
+                                                         int64_t n_tiles, const float2* __restrict__ rowp, const float* __restrict__ rad,
+                                                         const unsigned int* __restrict__ maxnorm_bits, uint32_t* __restrict__ words,
+                                                         int64_t n_words, int32_t* __restrict__ list_len) {
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
+  __shared__ float rs[CN];
+  __shared__ uint32_t surv[NSUB];
+  const uint32_t tile_b = (uint32_t)(CN * 16 * 2) * (uint32_t)nks;
+  unsigned char* As = smem_raw;
+  unsigned char* Bs = smem_raw + tile_b;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = warp >> 2, sl = lane & 3;
+  const float s = tc_scale_from_maxnorm(*maxnorm_bits);
+  {
+    const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(Aimg) + (size_t)blockIdx.x * tile_b);
+    uint4* dst = reinterpret_cast<uint4*>(As);
+    for (uint32_t i = threadIdx.x; i < tile_b / 16; i += blockDim.x) dst[i] = src[i];
+  }
+  if (threadIdx.x < NSUB) surv[threadIdx.x] = 0u;
+  const int row0 = 64 * g + 16 * (warp & 3) + (lane >> 2);
+  const float2 p0 = rowp[(int64_t)blockIdx.x * QM + row0], p1 = rowp[(int64_t)blockIdx.x * QM + row0 + 8];
+  const uint64_t da0 = wgmma_desc(smem_u32(As) + (uint32_t)g * 8u * SBO, LBO, SBO);
+  const uint64_t db0 = wgmma_desc(smem_u32(Bs), LBO, SBO);
+  constexpr uint32_t KSTEP16 = (2u * LBO) >> 4;
+  constexpr float C = 1.0f + 1.0f / 65536.0f;
+  uint32_t* out = words + (int64_t)blockIdx.x * n_words;
+  int32_t cnt = 0;   // warp 0: tiles kept so far
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+  const int64_t n_ct = (n_tiles + CN - 1) / CN;
+  for (int64_t ct = 0; ct < n_ct; ++ct) {
+    __syncthreads();   // the previous centre tile is no longer read
+    {
+      const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(Cimg) + (size_t)ct * tile_b);
+      uint4* dst = reinterpret_cast<uint4*>(Bs);
+      for (uint32_t i = threadIdx.x; i < tile_b / 16; i += blockDim.x) dst[i] = src[i];
+      if (threadIdx.x < CN) rs[threadIdx.x] = ct * CN + threadIdx.x < n_tiles ? rad[ct * CN + threadIdx.x] * s : 0.0f;
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic stores -> wgmma operand reads
+    __syncthreads();
+    wgmma_fence_operand(acc);
+    wgmma_fence();
+    for (int j = 0; j < nks; ++j)
+      wgmma_m64n128k16_f16(acc, da0 + (uint64_t)((uint32_t)j * KSTEP16), db0 + (uint64_t)((uint32_t)j * KSTEP16), j != 0);
+    wgmma_commit();
+    wgmma_wait_all();
+    wgmma_fence_operand(acc);
+    uint32_t keep = 0u;   // bit 2i + e: column 8i + 2 sl + e
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const float r = rs[8 * i + 2 * sl + e];
+        const float t0 = p0.y + r, t1 = p1.y + r;
+        const bool k0 = !(fmaf(-2.0f, acc[4 * i + e], p0.x) > t0 * t0 * C);
+        const bool k1 = !(fmaf(-2.0f, acc[4 * i + 2 + e], p1.x) > t1 * t1 * C);
+        keep |= (uint32_t)(k0 || k1) << (2 * i + e);
+      }
+    }
+    keep |= __shfl_xor_sync(0xffffffffu, keep, 4);
+    keep |= __shfl_xor_sync(0xffffffffu, keep, 8);
+    keep |= __shfl_xor_sync(0xffffffffu, keep, 16);
+    if (lane < NSUB) atomicOr(&surv[lane], keep);
+    __syncthreads();
+    if (warp == 0) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int col = lane + 32 * e;
+        const int64_t tile = ct * CN + col;
+        const bool f = tile < n_tiles && ((surv[(col >> 1) & 3] >> (2 * (col >> 3) + (col & 1))) & 1u);
+        const unsigned bal = __ballot_sync(0xffffffffu, f);
+        if (lane == 0 && ct * 4 + e < n_words) out[ct * 4 + e] = bal;
+        cnt += __popc(bal);
+      }
+    }
+    __syncthreads();
+    if (threadIdx.x < NSUB) surv[threadIdx.x] = 0u;
+  }
+  if (threadIdx.x == 0) {
+    if (cnt == 0) { out[0] |= 1u; cnt = 1; }   // only padding rows: the sweep needs one visit
+    list_len[blockIdx.x] = cnt;
+  }
+}
+
+// one warp per block: the set bits of its bitmap, ascending, to lists[off[block] ..]
+__global__ void knn_expand_lists_kernel(const uint32_t* __restrict__ words, int64_t n_words, int64_t n_blocks,
+                                        const int64_t* __restrict__ off, int32_t* __restrict__ lists) {
+  const int64_t b = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= n_blocks) return;
+  const int lane = threadIdx.x & 31;
+  int32_t* out = lists + off[b];
+  int64_t base = 0;
+  for (int64_t w0 = 0; w0 < n_words; w0 += 32) {
+    uint32_t w = w0 + lane < n_words ? words[b * n_words + w0 + lane] : 0u;
+    const int c = __popc(w);
+    int incl = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += t;
+    }
+    int64_t pos = base + incl - c;
+    while (w) {
+      out[pos++] = (int32_t)((w0 + lane) * 32 + __ffs(w) - 1);
+      w &= w - 1;
+    }
+    base += __shfl_sync(0xffffffffu, incl, 31);
+  }
+}
+
 }  // namespace
 
 bool knn_tc2_supported(int d) { return 3 * d + 3 <= 512; }
@@ -639,6 +1005,99 @@ int32_t knn_tc2_build_images(sb2_ctx* ctx, const KnnTc2Shape& sh, const float* d
   return SB2_OK;
 }
 
+
+int32_t knn_tc2_kd_order(sb2_ctx* ctx, const float* d_x, int64_t n, int d, int32_t* perm) {
+  cudaStream_t st = ctx->stream;
+  // the segments of every level depend on n alone: [a, b) splits at a + 128 * floor(tiles / 2)
+  std::vector<int32_t> segs;
+  std::vector<std::pair<size_t, int>> levels;   // (first segment, segments)
+  std::vector<std::pair<int64_t, int64_t>> cur{{0, n}}, nxt;
+  int max_seg = 0;
+  for (;;) {
+    nxt.clear();
+    const size_t first = segs.size() / 3;
+    for (const auto& ab : cur) {
+      if (ab.second - ab.first <= CN) continue;
+      const int64_t m = ab.first + CN * (ceil_div64(ab.second - ab.first, CN) / 2);
+      segs.insert(segs.end(), {(int32_t)ab.first, (int32_t)m, (int32_t)ab.second});
+      nxt.push_back({ab.first, m});
+      nxt.push_back({m, ab.second});
+    }
+    const int cnt = (int)(segs.size() / 3 - first);
+    if (cnt == 0) break;
+    levels.push_back({first, cnt});
+    max_seg = max_seg > cnt ? max_seg : cnt;
+    cur.swap(nxt);
+  }
+  kd_iota_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(perm, n);
+  SB2_LAUNCH_CHECK(ctx);
+  if (levels.empty()) return SB2_OK;
+  ScratchScope scr(ctx);
+  int32_t *d_segs, *axis, *other;
+  uint32_t* key;
+  SB2_TRY(scr.alloc(&d_segs, segs.size()));
+  SB2_TRY(scr.alloc(&axis, (size_t)max_seg));
+  SB2_TRY(scr.alloc(&other, (size_t)n));
+  SB2_TRY(scr.alloc(&key, (size_t)n));
+  SB2_CUDA(cudaMemcpyAsync(d_segs, segs.data(), segs.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  int32_t *src = perm, *dst = other;
+  for (const auto& lv : levels) {
+    const int32_t* sg = d_segs + lv.first * 3;
+    const unsigned ns = (unsigned)lv.second;
+    SB2_CUDA(cudaMemcpyAsync(dst, src, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));   // unsplit segments
+    kd_axis_kernel<<<ns, 256, 0, st>>>(d_x, d, src, sg, axis);
+    SB2_LAUNCH_CHECK(ctx);
+    kd_keys_kernel<<<dim3(ns, (unsigned)ceil_div64(2048, ns)), 256, 0, st>>>(d_x, d, src, sg, axis, key);
+    SB2_LAUNCH_CHECK(ctx);
+    kd_split_kernel<<<ns, KD_THREADS, 0, st>>>(sg, key, src, dst);
+    SB2_LAUNCH_CHECK(ctx);
+    int32_t* t = src; src = dst; dst = t;
+  }
+  if (src != perm) SB2_CUDA(cudaMemcpyAsync(perm, src, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  return SB2_OK;
+}
+
+int32_t knn_tc2_restrict(sb2_ctx* ctx, const int32_t* perm, int64_t n, int64_t q0, int64_t n_query, int32_t* qloc, int32_t* qpos) {
+  kd_restrict_kernel<<<1, KD_THREADS, 0, ctx->stream>>>(perm, n, q0, n_query, qloc, qpos);
+  SB2_LAUNCH_CHECK(ctx);
+  return SB2_OK;
+}
+
+int32_t knn_tc2_tile_stats(sb2_ctx* ctx, const float* d_x, int64_t n, int d, const int32_t* perm, const unsigned int* d_maxnorm_bits,
+                           float* cent, float* rad) {
+  kd_tile_stats_kernel<<<(unsigned)ceil_div64(n, CN), 256, 0, ctx->stream>>>(d_x, n, d, perm, d_maxnorm_bits, cent, rad);
+  SB2_LAUNCH_CHECK(ctx);
+  return SB2_OK;
+}
+
+int knn_tc2_near_tiles() { return NEAR_TILES; }
+
+int32_t knn_tc2_near_lists(sb2_ctx* ctx, int64_t n_blocks, int64_t n_tiles, const int32_t* qpos, int32_t* lists, int32_t* len) {
+  knn_near_lists_kernel<<<(unsigned)ceil_div64(n_blocks, 256), 256, 0, ctx->stream>>>(n_blocks, n_tiles, qpos, lists, len);
+  SB2_LAUNCH_CHECK(ctx);
+  return SB2_OK;
+}
+
+int64_t knn_tc2_screen_words(int64_t n_tiles) { return ceil_div64(n_tiles, 32); }
+
+int32_t knn_tc2_screen(sb2_ctx* ctx, const KnnTc2Shape& sh, const __half* Aimg, const __half* Cimg, int64_t n_blocks, int64_t n_tiles,
+                       const float2* rowp, const float* rad, const unsigned int* d_maxnorm_bits, uint32_t* words, int32_t* list_len) {
+  SB2_CHECK_ARG(sh.nsplit == 1, "the tile screen needs whole images in shared memory");
+  const size_t smem = (size_t)2 * QM * sh.kpad * 2;
+  SB2_CUDA(cudaFuncSetAttribute(knn_screen_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  knn_screen_kernel<<<(unsigned)n_blocks, 256, smem, ctx->stream>>>(Aimg, Cimg, sh.kpad / 16, n_tiles, rowp, rad, d_maxnorm_bits,
+                                                                    words, knn_tc2_screen_words(n_tiles), list_len);
+  SB2_LAUNCH_CHECK(ctx);
+  return SB2_OK;
+}
+
+int32_t knn_tc2_expand_lists(sb2_ctx* ctx, const uint32_t* words, int64_t n_blocks, int64_t n_tiles, const int64_t* off, int32_t* lists) {
+  knn_expand_lists_kernel<<<(unsigned)ceil_div64(n_blocks, 8), 256, 0, ctx->stream>>>(words, knn_tc2_screen_words(n_tiles), n_blocks,
+                                                                                      off, lists);
+  SB2_LAUNCH_CHECK(ctx);
+  return SB2_OK;
+}
+
 namespace {
 // f(NG, PNKS, STAMPS, ISCAN) as std::integral_constants, the template arguments of knn_sweep2_kernel: NG = 2 for lists of
 // 64 proposals, 4 for 128; PNKS the pipelined loop's k-steps when pipe (knn_tc2_shape only sets it for nsplit = 1 and
@@ -666,7 +1125,7 @@ void with_sweep2(int list_m, bool iscan, bool pipe, int kpad, bool stamps, F&& f
 
 // SB2_KNN_STAMPS=1: where the consumer warpgroups of one sweep spent their cycles, summed over all of them, and how
 // often they left the fast path, on stderr
-int32_t report_stamps(sb2_ctx* ctx, const KnnTc2Shape& sh, bool pipe, unsigned grid, int64_t n_visit, int64_t n_est, int64_t n_query,
+int32_t report_stamps(sb2_ctx* ctx, const KnnTc2Shape& sh, bool pipe, unsigned grid, double visits, double est_visits, int64_t n_query,
                       int list_m, const unsigned long long* d_stamps) {
   std::vector<unsigned long long> h((size_t)grid * 2 * ST_N);
   SB2_CUDA(cudaMemcpyAsync(h.data(), d_stamps, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
@@ -676,16 +1135,16 @@ int32_t report_stamps(sb2_ctx* ctx, const KnnTc2Shape& sh, bool pipe, unsigned g
     tot[i % ST_N] += (double)h[i];
     if (i % ST_N < PH_N) all += (double)h[i];
   }
-  const double tiles = (double)grid * 2.0 * (double)n_visit;   // tiles examined, counted per warpgroup
+  const double tiles = 2.0 * visits;   // tiles examined (all CTAs), counted per warpgroup
   static const char* names[PH_N] = {"wait full", "mma", "scan", "insert"};
-  fprintf(stderr, "[sb2 knn stamps] %s loop, K=%d nsplit=%d nstage=%d list=%d, %u CTAs x %lld visits: %.0f cycles/tile",
-          pipe ? "pipelined" : "single-buffer", sh.kpad, sh.nsplit, sh.nstage, list_m, grid, (long long)n_visit,
+  fprintf(stderr, "[sb2 knn stamps] %s loop, K=%d nsplit=%d nstage=%d list=%d, %u CTAs x %.1f visits: %.0f cycles/tile",
+          pipe ? "pipelined" : "single-buffer", sh.kpad, sh.nsplit, sh.nstage, list_m, grid, grid ? visits / grid : 0.0,
           tiles > 0 ? all / tiles : 0.0);
   for (int ph = 0; ph < PH_N; ++ph)
     fprintf(stderr, ", %s %.1f%% (%.0f)", names[ph], all > 0 ? 100.0 * tot[ph] / all : 0.0, tiles > 0 ? tot[ph] / tiles : 0.0);
   // the rare path: share of the sweep proper's warp-tiles (8 consumer warps per CTA) on which a warp took it, and the
   // insertions per query row (four sub-lists)
-  const double warp_tiles = (double)grid * NCONS * (double)(n_visit - n_est);
+  const double warp_tiles = NCONS * (visits - est_visits);
   fprintf(stderr, ", rare-path tiles %.2f%%, insertions/row %.1f\n", warp_tiles > 0 ? 100.0 * tot[CNT_RARE] / warp_tiles : 0.0,
           n_query > 0 ? tot[CNT_INSERT] / (double)n_query : 0.0);
   return SB2_OK;
@@ -694,7 +1153,7 @@ int32_t report_stamps(sb2_ctx* ctx, const KnnTc2Shape& sh, bool pipe, unsigned g
 
 int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnSwitches& sw, const KnnTc2Shape& sh, const __half* Aimg, int64_t a_tile0,
                       const __half* Bimg, int64_t n_points, int64_t n_query, int list_m, float* cand_score, int32_t* cand_idx,
-                      double* issued_flops) {
+                      double* issued_flops, const KnnTc2Lists* lists) {
   cudaStream_t st = ctx->stream;
   const int64_t n_tiles = ceil_div64(n_points, CN);
   const int64_t q_ctas = ceil_div64(n_query, QM);
@@ -703,13 +1162,25 @@ int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnSwitches& sw, const KnnTc2Shape& sh
   // rank est_rank * est_stride of the row
   const int64_t est_stride = sw.est_stride;
   int64_t n_est = sw.cold ? 0 : n_tiles / est_stride;
-  if (n_tiles < 32 * est_stride || !sh.est) n_est = 0;  // small problems / split-precision sweeps: cold start
+  if (n_tiles < 32 * est_stride || !sh.est || lists) n_est = 0;  // small problems / split-precision sweeps / tile lists
   // the sub-lists start at the est_rank-th largest of the row's sampled chunk maxima, rank ~96 of the row by default:
   // on the 1.3M x 50 benchmark (k = 15) every rank below 6 sends more rows to the split-precision re-sweep (rank 5:
   // 7x as many, rank 4: 46x) than it saves in insertions.  SB2_KNN_EST_RANK=1..6 picks another (tests, A/B timing).
   const int est_rank = sw.est_rank;
-  if (issued_flops) *issued_flops += 2.0 * (double)(q_ctas * QM) * (double)((n_tiles + n_est) * CN) * (double)sh.kpad;
   const unsigned grid = (unsigned)q_ctas;
+  ScratchScope scr(ctx);
+  // without tile lists every CTA walks all tiles: one shared identity list
+  KnnTc2Lists all{nullptr, 0, nullptr, nullptr, q_ctas * n_tiles, nullptr, sw.stamps};
+  if (!lists) {
+    int32_t* ident;
+    SB2_TRY(scr.alloc(&ident, (size_t)n_tiles));
+    kd_iota_kernel<<<(unsigned)ceil_div64(n_tiles, 256), 256, 0, st>>>(ident, n_tiles);
+    SB2_LAUNCH_CHECK(ctx);
+    all.idx = ident;
+    lists = &all;
+  }
+  const double visits = (double)lists->total + (double)q_ctas * (double)n_est;
+  if (issued_flops) *issued_flops += 2.0 * QM * visits * CN * (double)sh.kpad;
   const int32_t np = (int32_t)n_points;
   {
     void* fp = nullptr;
@@ -718,24 +1189,23 @@ int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnSwitches& sw, const KnnTc2Shape& sh
   }
   // SB2_KNN_PIPE=0 and SB2_KNN_SCAN=float give the same results (A/B timing)
   const bool pipe = sh.pipe && sw.pipe;
-  ScratchScope scr(ctx);
   unsigned long long* stamps = nullptr;
-  if (sw.stamps) {
+  if (lists->stamps) {
     SB2_TRY(scr.alloc(&stamps, (size_t)grid * 2 * ST_N));
     SB2_CUDA(cudaMemsetAsync(stamps, 0, (size_t)grid * 2 * ST_N * sizeof(unsigned long long), st));
   }
   cudaError_t le = cudaSuccess;
-  with_sweep2(list_m, sw.int_scan, pipe, sh.kpad, sw.stamps, [&](auto ng, auto pnks, auto st_on, auto iscan) {
+  with_sweep2(list_m, sw.int_scan, pipe, sh.kpad, lists->stamps, [&](auto ng, auto pnks, auto st_on, auto iscan) {
     le = cudaFuncSetAttribute(knn_sweep2_kernel<ng, pnks, st_on, iscan>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sh.smem);
     if (le != cudaSuccess) return;
     const int nks = sh.kpad / 16 / sh.nsplit;
     knn_sweep2_kernel<ng, pnks, st_on, iscan><<<grid, pnks > 0 ? THREADS_PIPE : THREADS, sh.smem, st>>>(
-        Aimg, Bimg, nks, sh.nsplit, sh.nstage, n_tiles, n_est, est_stride, est_rank, a_tile0, n_query, np, cand_score, cand_idx,
-        stamps);
+        Aimg, Bimg, nks, sh.nsplit, sh.nstage, n_tiles, n_est, est_stride, est_rank, a_tile0, n_query, np, lists->idx, lists->stride,
+        lists->off, lists->len, lists->seed, cand_score, cand_idx, stamps);
   });
   SB2_CUDA(le);
   SB2_LAUNCH_CHECK(ctx);
-  if (stamps) SB2_TRY(report_stamps(ctx, sh, pipe, grid, n_tiles + n_est, n_est, n_query, list_m, stamps));
+  if (stamps) SB2_TRY(report_stamps(ctx, sh, pipe, grid, visits, (double)q_ctas * (double)n_est, n_query, list_m, stamps));
   return SB2_OK;
 }
 
