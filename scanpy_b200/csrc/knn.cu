@@ -608,6 +608,11 @@ KnnSwitches knn_switches() {
   s.int_scan = !is("SB2_KNN_SCAN", "float");
   if (is("SB2_KNN_SCREEN", "0")) s.screen = 0;
   else if (is("SB2_KNN_SCREEN", "1")) s.screen = 1;
+  if (const char* e = getenv("SB2_KNN_NEAR")) {   // anything but 1..KNN_MAX_NEAR fails the screened call (screen_prep)
+    char* end = nullptr;
+    const long v = strtol(e, &end, 10);
+    s.near_tiles = (end != e && *end == '\0' && v >= 1 && v <= KNN_MAX_NEAR) ? (int)v : 0;
+  }
   return s;
 }
 
@@ -738,9 +743,11 @@ int32_t sweep_and_certify(KnnCall& c, const Tier& t, const __half* A, int64_t a_
 // Above this share of kept (block, tile) pairs the screen's lists are dropped for the full sweep (SB2_KNN_SCREEN=1 keeps
 // them): see DESIGN.md §4 for the measurement behind it.
 constexpr double SCREEN_MAX_KEPT = 0.9;
+constexpr int NEAR_COLD = 8;   // tiles of the screen's cold short sweep (the rest of the near tiles are swept seeded)
 
 // Tier 1's images in the kd order and the tile screen: the order, the per-tile centres and radii, a short sweep of each
-// block's own neighbourhood (NEAR_TILES tiles) whose proposals bound every row's k-th distance (knn_row_bound_kernel),
+// block's own neighbourhood (SB2_KNN_NEAR consecutive tiles, 64 by default: a cold pass over the middle NEAR_COLD of
+// them, then a pass over all of them seeded from its bound) whose proposals bound every row's k-th distance (knn_row_bound_kernel),
 // then the screen of every row against every tile centre (knn_screen_kernel).  Bracketed by the call's events, so the
 // reported sweep time includes it; SB2_KNN_STAMPS=1 reports its parts.  The lists are kept (S.lists) when they skip
 // enough tiles (SCREEN_MAX_KEPT) and fit in device memory, or always with `force`; otherwise S.lists stays nullptr and
@@ -785,19 +792,25 @@ int32_t screen_prep(KnnCall& c, Tier& t1, __half* A1, float* inv_s2, float* dnor
   SB2_TRY(scr.alloc(&Cimg, knn_tc2_b_halves(t1.sh, n_tiles)));
   SB2_TRY(knn_tc2_tile_stats(ctx, c.d_x, n_points, d, S.perm, c.maxnorm, cent, rad));
   SB2_TRY(knn_tc2_build_images(ctx, t1.sh, cent, n_tiles, d, c.maxnorm, nullptr, 0, nullptr, Cimg, inv_s2));
-  // the short sweep: cold, over each block's own neighbourhood
-  const int nt = knn_tc2_near_tiles();
-  int32_t *near, *near_len;
-  SB2_TRY(scr.alloc(&near, (size_t)n_blocks * nt));
-  SB2_TRY(scr.alloc(&near_len, (size_t)n_blocks));
-  SB2_TRY(knn_tc2_near_lists(ctx, n_blocks, n_tiles, S.qpos, near, near_len));
-  const KnnTc2Lists NL{near, nt, nullptr, near_len, n_blocks * (nt < n_tiles ? nt : n_tiles), nullptr, false};
-  SB2_TRY(knn_tc2_sweep(ctx, c.sw, t1.sh, A1, 0, t1.B, n_points, n_query, c.list_m, c.cand_score, c.cand_idx, &c.issued_flops, &NL));
+  // the short sweep over each block's own neighbourhood, nt consecutive tiles of the order (64 by default, not 8: a
+  // block at a split boundary has its neighbours across the split, far away in the order; DESIGN.md §4).  A cold
+  // sweep inserts on nearly every tile, so it covers only the middle NEAR_COLD tiles; its bound u1 seeds a second
+  // sweep over all nt.  Every point within u1 scores above the seed, so the second sweep's sub-lists keep every
+  // proposal a cold sweep of the nt tiles would rank in the top k (the k from the first sweep among them): its u is
+  // the cold sweep's, at the cost of a warm sweep.
+  const int nt = c.sw.near_tiles;
+  SB2_CHECK_ARG(nt >= 1 && nt <= KNN_MAX_NEAR, "SB2_KNN_NEAR must be an integer in 1..64");
   float2* rowp;
   SB2_TRY(scr.alloc(&S.ub, (size_t)n_query));
   SB2_TRY(scr.alloc(&S.seed, (size_t)n_query));
   SB2_TRY(scr.alloc(&rowp, (size_t)n_blocks * TILE));
-  {
+  int32_t *near, *near_len;
+  SB2_TRY(scr.alloc(&near, (size_t)n_blocks * nt));
+  SB2_TRY(scr.alloc(&near_len, (size_t)n_blocks));
+  const auto short_sweep = [&](int w, const float* seed) -> int32_t {
+    SB2_TRY(knn_tc2_near_lists(ctx, n_blocks, n_tiles, w, S.qpos, near, near_len));
+    const KnnTc2Lists NL{near, w, nullptr, near_len, n_blocks * (w < n_tiles ? w : n_tiles), seed, false};
+    SB2_TRY(knn_tc2_sweep(ctx, c.sw, t1.sh, A1, 0, t1.B, n_points, n_query, c.list_m, c.cand_score, c.cand_idx, &c.issued_flops, &NL));
     const int wpb = 8;
     const int64_t n_pad = n_blocks * TILE;
     const unsigned grid = (unsigned)ceil_div64(n_pad, wpb);
@@ -809,7 +822,10 @@ int32_t screen_prep(KnnCall& c, Tier& t1, __half* A1, float* inv_s2, float* dnor
     if (c.list_m == 64) launch(std::integral_constant<int, 2>());
     else launch(std::integral_constant<int, 4>());
     SB2_LAUNCH_CHECK(ctx);
-  }
+    return SB2_OK;
+  };
+  SB2_TRY(short_sweep(nt < NEAR_COLD ? nt : NEAR_COLD, nullptr));
+  if (nt > NEAR_COLD) SB2_TRY(short_sweep(nt, S.seed));
   // the screen writes a bitmap per block (n_tiles / 8 bytes) and its count; only the kept tiles become list entries
   uint32_t* words;
   SB2_TRY(scr.alloc(&words, (size_t)n_blocks * knn_tc2_screen_words(n_tiles)));
@@ -845,8 +861,8 @@ int32_t screen_prep(KnnCall& c, Tier& t1, __half* A1, float* inv_s2, float* dnor
     std::vector<int32_t> v = S.h_len;
     std::sort(v.begin(), v.end());
     fprintf(stderr, "[sb2 knn screen] %lld blocks x %lld tiles: surviving %.4f, list length min %d median %d max %d; kd order %.2f ms, "
-            "images + short sweep + screen %.2f ms; %s\n", (long long)n_blocks, (long long)n_tiles, kept, v.front(), v[v.size() / 2],
-            v.back(), ms_order, ms_screen, S.lists ? "tile lists" : "full sweep (too few tiles skipped, or lists do not fit)");
+            "images + short sweep (%d near tiles) + screen %.2f ms; %s\n", (long long)n_blocks, (long long)n_tiles, kept, v.front(),
+            v[v.size() / 2], v.back(), ms_order, nt, ms_screen, S.lists ? "tile lists" : "full sweep (too few tiles skipped, or lists do not fit)");
   }
   return SB2_OK;
 }

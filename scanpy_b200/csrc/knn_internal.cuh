@@ -6,6 +6,7 @@
 
 constexpr int EST_R = 6;           // chunk maxima an estimate keeps per (row, sub-list)
 constexpr int EST_STRIDE = 16;     // the estimate samples every 16th candidate tile
+constexpr int KNN_MAX_NEAR = 64;   // longest near list of the tile screen's short sweep (SB2_KNN_NEAR)
 
 // float <-> unsigned with the same order (the kd order's radix select, the k-th largest proposal score)
 __device__ __forceinline__ uint32_t ord_bits(float x) {
@@ -28,6 +29,7 @@ struct KnnSwitches {
   bool stamps = false;          // SB2_KNN_STAMPS=1: each sweep launch reports its consumers' cycle split on stderr
   bool int_scan = true;         // SB2_KNN_SCAN=float (false): the float max tree in the fast path of the sweep's examination
   int screen = -1;              // SB2_KNN_SCREEN=0: no tile screen; =1: screen at every size; unset: from 512 candidate tiles
+  int near_tiles = 64;          // SB2_KNN_NEAR=1..KNN_MAX_NEAR: consecutive tiles of the kd order in the screen's short sweep
 };
 
 // ---- tensor-core sweep (knn_tc2.cu): 128-query CTAs x 128-candidate tiles (wgmma N = 128), two consumer warpgroups,
@@ -76,9 +78,8 @@ int32_t knn_tc2_restrict(sb2_ctx* ctx, const int32_t* perm, int64_t n, int64_t q
 // per tile of perm: cent[t * d ..] the centre (fp16-exact in the images' scale), rad[t] >= max |x - cent_t|
 int32_t knn_tc2_tile_stats(sb2_ctx* ctx, const float* d_x, int64_t n, int d, const int32_t* perm, const unsigned int* d_maxnorm_bits,
                            float* cent, float* rad);
-int knn_tc2_near_tiles();
-// lists [n_blocks][near_tiles]: the consecutive tiles around the tile of each block's first row (qpos == nullptr: row = position)
-int32_t knn_tc2_near_lists(sb2_ctx* ctx, int64_t n_blocks, int64_t n_tiles, const int32_t* qpos, int32_t* lists, int32_t* len);
+// lists [n_blocks][nt]: the nt consecutive tiles around the tile of each block's first row (qpos == nullptr: row = position)
+int32_t knn_tc2_near_lists(sb2_ctx* ctx, int64_t n_blocks, int64_t n_tiles, int nt, const int32_t* qpos, int32_t* lists, int32_t* len);
 // per query block of Aimg the tiles some row may need (rowp: see knn_screen_kernel): a bitmap of
 // knn_tc2_screen_words(n_tiles) words per block and the count of its set bits
 int64_t knn_tc2_screen_words(int64_t n_tiles);

@@ -631,7 +631,6 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
 // tile holds no point within u(q) of any row of the block; the re-score checks d_k(q) <= u(q) before it certifies a row.
 constexpr int KD_SAMPLES = 512;   // points per segment the split coordinate is chosen from
 constexpr int KD_THREADS = 1024;
-constexpr int NEAR_TILES = 8;     // tiles of the short sweep that gives u(q): the block's own tile and its neighbours
 
 // segment s of a level = [seg[3s], seg[3s+2]), split at seg[3s+1]: its coordinate of largest variance over an evenly
 // spaced sample of its points (any choice is correct; the variance only makes the tiles tight)
@@ -826,15 +825,15 @@ __global__ void __launch_bounds__(256) kd_tile_stats_kernel(const float* __restr
   if (threadIdx.x == 0) rad[t] = __uint_as_float(rmax);
 }
 
-// the short sweep's lists: NEAR_TILES consecutive tiles of the order around the tile of the block's first row
-__global__ void knn_near_lists_kernel(int64_t n_blocks, int64_t n_tiles, const int32_t* __restrict__ qpos, int32_t* __restrict__ lists,
-                                      int32_t* __restrict__ len) {
+// the short sweep's lists: nt consecutive tiles of the order around the tile of the block's first row
+__global__ void knn_near_lists_kernel(int64_t n_blocks, int64_t n_tiles, int nt, const int32_t* __restrict__ qpos,
+                                      int32_t* __restrict__ lists, int32_t* __restrict__ len) {
   const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= n_blocks) return;
   const int64_t own = (qpos ? (int64_t)qpos[b * QM] : b * QM) / CN;
-  const int64_t cnt = min((int64_t)NEAR_TILES, n_tiles);
-  const int64_t first = max((int64_t)0, min(own - NEAR_TILES / 2 + 1, n_tiles - cnt));
-  for (int64_t i = 0; i < cnt; ++i) lists[b * NEAR_TILES + i] = (int32_t)(first + i);
+  const int64_t cnt = min((int64_t)nt, n_tiles);
+  const int64_t first = max((int64_t)0, min(own - (nt - 1) / 2, n_tiles - cnt));
+  for (int64_t i = 0; i < cnt; ++i) lists[b * nt + i] = (int32_t)(first + i);
   len[b] = (int32_t)cnt;
 }
 
@@ -1070,10 +1069,9 @@ int32_t knn_tc2_tile_stats(sb2_ctx* ctx, const float* d_x, int64_t n, int d, con
   return SB2_OK;
 }
 
-int knn_tc2_near_tiles() { return NEAR_TILES; }
-
-int32_t knn_tc2_near_lists(sb2_ctx* ctx, int64_t n_blocks, int64_t n_tiles, const int32_t* qpos, int32_t* lists, int32_t* len) {
-  knn_near_lists_kernel<<<(unsigned)ceil_div64(n_blocks, 256), 256, 0, ctx->stream>>>(n_blocks, n_tiles, qpos, lists, len);
+int32_t knn_tc2_near_lists(sb2_ctx* ctx, int64_t n_blocks, int64_t n_tiles, int nt, const int32_t* qpos, int32_t* lists, int32_t* len) {
+  SB2_CHECK_ARG(nt >= 1 && nt <= KNN_MAX_NEAR, "near tiles");
+  knn_near_lists_kernel<<<(unsigned)ceil_div64(n_blocks, 256), 256, 0, ctx->stream>>>(n_blocks, n_tiles, nt, qpos, lists, len);
   SB2_LAUNCH_CHECK(ctx);
   return SB2_OK;
 }
