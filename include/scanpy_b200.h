@@ -357,6 +357,35 @@ int32_t sb2_autocorr_sums(sb2_ctx* ctx, int64_t row0, int64_t rows, int32_t g, i
                           const double* d_mean, double* d_acc);
 
 
+/* ---- sc.get.aggregate (src/scanpy/get/_aggregated.py:47-190, 663-698; csrc/aggregate.cu) ----
+ * sb2_aggregate_group_order <- the stable order of the kept rows by group: d_codes int32 [n] in [0, n_groups) or -1 (no
+ *                              group); d_offsets int64 [n_groups + 1] = each group's first position (d_offsets[n_groups]
+ *                              = kept rows) and d_order int64 [>= kept rows] the row ids, each group's rows ascending.
+ * X is dense (d_x, row-major [rows x g]) or CSR arrays (sorted column indices, no duplicates), float32 (is_f64 = 0) or
+ * float64 values; row k of a call is X row d_order[k] (d_order NULL: row k).  The call's rows form n_seg segments,
+ * segment s = call rows h_seg_row[s] .. h_seg_row[s + 1] - 1 (host arrays), consecutive rows of group h_seg_group[s];
+ * a group appears in at most one segment per call.
+ * sb2_aggregate_moments <- Aggregate.sum / mean_var / count_nonzero: merges each segment's rows into its group's row
+ *                          of d_sum, d_mean, d_m2 (fp64 [n_groups x g]: Σx, the mean, the sum of squared deviations)
+ *                          and d_nnz (int64: the count of x != 0; implicit and stored zeros are zeros).  h_seg_n0[s] =
+ *                          the group's rows merged by earlier calls, a multiple of SB2_AGGREGATE_TILE_ROWS (0: the
+ *                          group's outputs are overwritten).  The bits depend only on each group's rows and their order.
+ * sb2_aggregate_median  <- Aggregate.median: d_out [n_groups x g] (float32 when is_f64 = 0, else float64) row
+ *                          h_seg_group[s] = np.median over the segment's rows, which must be all of the group's rows:
+ *                          the mean, in the value type, of the order statistics (n-1)/2 and n/2 with zeros included.
+ *                          A CSR's NaN sorts above +inf (sklearn's csc_median_axis_0); a dense group with a NaN gives
+ *                          NaN (np.median). */
+#define SB2_AGGREGATE_TILE_ROWS 1024
+int32_t sb2_aggregate_group_order(sb2_ctx* ctx, int64_t n, const int32_t* d_codes, int32_t n_groups,
+                                  int64_t* d_order, int64_t* d_offsets);
+int32_t sb2_aggregate_moments(sb2_ctx* ctx, int32_t n_seg, const int64_t* h_seg_row, const int32_t* h_seg_group,
+                              const int64_t* h_seg_n0, int32_t g, int32_t is_f64, const void* d_x,
+                              const int64_t* d_indptr, const int32_t* d_indices, const void* d_data,
+                              const int64_t* d_order, double* d_sum, double* d_mean, double* d_m2, int64_t* d_nnz);
+int32_t sb2_aggregate_median(sb2_ctx* ctx, int32_t n_seg, const int64_t* h_seg_row, const int32_t* h_seg_group,
+                             int32_t g, int32_t is_f64, const void* d_x, const int64_t* d_indptr,
+                             const int32_t* d_indices, const void* d_data, const int64_t* d_order, void* d_out);
+
 /* ---- extreme eigenpairs of diag(s) A diag(s), A symmetric fp32 CSR (csrc/eigs.cu: thick-restart Lanczos, fp64) ----
  * Replaces `scipy.sparse.linalg.eigsh(matrix.astype(float64), k=n_comps, which='LM', v0=...)` in
  * Neighbors.compute_eigen (src/scanpy/neighbors/__init__.py:832-884; sc.tl.diffmap) and the eigsh of umap's spectral

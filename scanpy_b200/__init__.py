@@ -7,7 +7,7 @@ writes `.obsm['X_pca']`, `.varm['PCs']`, `.uns['pca']`, `.obsp['distances'|'conn
 `.uns['neighbors']`, `.obs['leiden']`, `.uns['leiden']` exactly as scanpy does.  All arithmetic runs
 in hand-written CUDA behind the C ABI in include/scanpy_b200.h; there is no CPU fallback.
 """
-from . import experimental, metrics, pp, tl  # noqa: F401
+from . import experimental, get, metrics, pp, tl  # noqa: F401
 from ._compat import MiniAnnData, settings  # noqa: F401
 from ._io import ZarrCSR, read_zarr_backed  # noqa: F401
 from .transformer import B200KNNTransformer, B200PCA  # noqa: F401

@@ -160,6 +160,12 @@ SIGNATURES = {
                                     c_int32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "sb2_autocorr_sums": (c_int32, [c_void_p, c_int64, c_int64, c_int32, c_int32, c_void_p, c_void_p, c_void_p, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "sb2_aggregate_group_order": (c_int32, [c_void_p, c_int64, c_void_p, c_int32, c_void_p, c_void_p]),
+    "sb2_aggregate_moments": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p,
+                                        c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        c_void_p]),
+    "sb2_aggregate_median": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

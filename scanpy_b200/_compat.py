@@ -87,35 +87,47 @@ class _AxisArrays(dict):
 class MiniAnnData:
     """Minimal AnnData look-alike: enough surface for pca/neighbors/leiden and their tests."""
 
-    def __init__(self, X=None, obs=None, var=None, obsm=None, varm=None, obsp=None, uns=None):
+    def __init__(self, X=None, obs=None, var=None, obsm=None, varm=None, obsp=None, uns=None, layers=None):
         self.X = X
-        n_obs, n_vars = X.shape
+        self.layers = dict(layers or {})
+        n_obs, n_vars = self.shape if X is not None or self.layers else (len(obs), len(var))
         self.obs = obs if obs is not None else pd.DataFrame(index=pd.RangeIndex(n_obs).astype(str))
         self.var = var if var is not None else pd.DataFrame(index=pd.RangeIndex(n_vars).astype(str))
         self.obsm = _AxisArrays(obsm or {})
         self.varm = _AxisArrays(varm or {})
         self.obsp = _AxisArrays(obsp or {})
         self.uns = dict(uns or {})
-        self.layers = {}
         self.is_view = False
         self.isbacked = False
 
     @property
     def shape(self):
-        return self.X.shape
+        """X's shape; with X None (a result made of layers only, like `get.aggregate`'s) the first layer's, else
+        (len(obs), len(var))."""
+        if self.X is not None:
+            return self.X.shape
+        if self.layers:
+            return next(iter(self.layers.values())).shape
+        return (len(self.obs), len(self.var))
 
     @property
     def n_obs(self):
-        return self.X.shape[0]
+        return self.shape[0]
 
     @property
     def n_vars(self):
-        return self.X.shape[1]
+        return self.shape[1]
+
+    @property
+    def T(self):
+        """The transpose: X and layers transposed, obs / var and obsm / varm swapped (obsp and uns are not carried)."""
+        return MiniAnnData(None if self.X is None else self.X.T, self.var, self.obs, dict(self.varm), dict(self.obsm),
+                           layers={k: v.T for k, v in self.layers.items()})
 
     def copy(self):
         import copy
 
-        new = MiniAnnData(self.X.copy(), self.obs.copy(), self.var.copy(),
+        new = MiniAnnData(None if self.X is None else self.X.copy(), self.obs.copy(), self.var.copy(),
                           {k: v.copy() for k, v in self.obsm.items()}, {k: v.copy() for k, v in self.varm.items()},
                           {k: v.copy() for k, v in self.obsp.items()}, copy.deepcopy(self.uns))
         new.layers = {k: v.copy() for k, v in self.layers.items()}

@@ -1,4 +1,5 @@
-// slab.cuh — the column-slab scheme of the dense per-gene passes (regress.cu, pearson.cu, combat.cu, autocorr.cu).
+// slab.cuh — the column-slab scheme of the dense per-gene passes (regress.cu, pearson.cu, combat.cu, autocorr.cu,
+// aggregate.cu).
 //
 // One CTA owns a SLAB_THREADS-column slab of a block of rows and each thread one column.  A CSR input is read in place:
 // the CTA binary-searches its slab in each of SLAB_ROWS rows (column indices sorted, no duplicates) and scatters the
@@ -17,7 +18,8 @@ constexpr int SLAB_THREADS = 256;  // one column per thread: 256-column slabs
 constexpr int SLAB_ROWS = 16;      // rows staged per step
 constexpr int SLAB_TILE = 1024;    // rows per subtile
 static_assert(SLAB_TILE == SB2_REGRESS_TILE_ROWS && SLAB_TILE == SB2_PEARSON_TILE_ROWS &&
-              SLAB_TILE == SB2_COMBAT_TILE_ROWS && SLAB_TILE == SB2_AUTOCORR_TILE_ROWS && SLAB_TILE % SLAB_ROWS == 0,
+              SLAB_TILE == SB2_COMBAT_TILE_ROWS && SLAB_TILE == SB2_AUTOCORR_TILE_ROWS &&
+              SLAB_TILE == SB2_AGGREGATE_TILE_ROWS && SLAB_TILE % SLAB_ROWS == 0,
               "subtile");
 
 // The slab [c0, c1) of the m rows rid[0..m) of a CSR, scattered into tile[r][col - c0]; tile must be zero on entry.
