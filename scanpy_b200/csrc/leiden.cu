@@ -179,22 +179,27 @@ decide_kernel(Level L, const int32_t* __restrict__ wl, int32_t w_begin, int32_t 
       else if (allowed(c)) { best_gain = (double)tot - scale * (double)K[c]; best = c; }
     }
   } else {
-    // hash slice [e0, e1): capacity = deg >= number of distinct neighbouring communities
-    for (int64_t s = e0 + lane; s < e1; s += 32) { hkeys[s] = -1; hvals[s] = 0; }
+    // hash slice [2 e0, 2 e1): capacity = 2 deg, at least twice the number of distinct neighbouring communities.  An
+    // aggregated row lists every neighbour once, so refinement's keys (refined labels, singletons at first) are nearly
+    // all distinct: at capacity deg the linear probing would run at load ~1 with probe chains that grow with the row.
+    // At load <= 1/2 they stay short (the slot order changes no sum and no arg-max, so the decisions are the same)
+    const int64_t h0 = 2 * e0, h1 = 2 * e1;
+    const uint32_t cap = (uint32_t)(h1 - h0);
+    for (int64_t s = h0 + lane; s < h1; s += 32) { hkeys[s] = -1; hvals[s] = 0; }
     __syncwarp();
     for (int64_t e = e0 + lane; e < e1; e += 32) {
       const int32_t u = L.indices[e];
       if (u == v || (REFINE && comm[u] != pv)) continue;
       const int32_t c = REFINE ? ref[u] : comm[u];
-      uint32_t slot = mix32((uint32_t)c) % (uint32_t)deg;
+      uint32_t slot = mix32((uint32_t)c) % cap;
       for (;;) {
-        const int32_t prev = atomicCAS(&hkeys[e0 + slot], -1, c);
-        if (prev == -1 || prev == c) { atomicAdd((u64*)&hvals[e0 + slot], (u64)L.w[e]); break; }
-        slot = slot + 1 == (uint32_t)deg ? 0 : slot + 1;
+        const int32_t prev = atomicCAS(&hkeys[h0 + slot], -1, c);
+        if (prev == -1 || prev == c) { atomicAdd((u64*)&hvals[h0 + slot], (u64)L.w[e]); break; }
+        slot = slot + 1 == cap ? 0 : slot + 1;
       }
     }
     __syncwarp();
-    for (int64_t s = e0 + lane; s < e1; s += 32) {
+    for (int64_t s = h0 + lane; s < h1; s += 32) {
       const int32_t c = hkeys[s];
       if (c < 0) continue;
       const double tot = (double)hvals[s];
@@ -476,8 +481,8 @@ struct Work {
   int32_t n0;
   u64* K;          // [n0]
   int32_t* csize;  // [n0]
-  int32_t* hkeys;  // [E0]
-  int64_t* hvals;  // [E0]
+  int32_t* hkeys;  // [2 E0]
+  int64_t* hvals;  // [2 E0]
   int32_t* target; // [n0]
   uint8_t* tsingle;
   int32_t* wl[2];     // work-lists (vertices to decide this sweep / next sweep)
@@ -495,6 +500,9 @@ struct Work {
   bool careful;     // small INPUT graphs (n0 < CAREFUL_N): 8 vertex classes per round of sweeps + independent-set rule - closer
                     // to the sequential algorithm, at a cost in sweeps that only a graph this small can afford
   bool exact;       // SB2_LEIDEN_EXACT=1: no first-pass / refinement cut-offs (every phase runs to its fixed point)
+  bool timing;      // SB2_TIMING set: per-level sweep / round counts on stderr
+  bool verbose;     // SB2_TIMING and SB2_VERBOSE set: one line per sweep
+  int64_t syncs;    // host synchronisations of the sweep loops and the aggregation (SB2_TIMING summary)
 };
 
 inline unsigned gridw(int64_t n) { return (unsigned)ceil_div64(n, 8); }    // warp per item, 8 warps/CTA
@@ -545,6 +553,7 @@ int32_t compact(Work& w, int32_t n, const int32_t* src, int32_t* out, int32_t* n
   SB2_CUDA(cudaMemcpyAsync(&cnt, w.pos + n, sizeof(int64_t), cudaMemcpyDeviceToHost, w.st));
   if (counter0) SB2_CUDA(cudaMemcpyAsync(counter0, w.counter, sizeof(u64), cudaMemcpyDeviceToHost, w.st));
   SB2_CUDA(cudaStreamSynchronize(w.st));
+  ++w.syncs;
   *n_out = (int32_t)cnt;
   return SB2_OK;
 }
@@ -577,7 +586,7 @@ int32_t local_move(Work& w, const Level& L, int32_t* comm, int64_t* moves_out) {
     SB2_TRY(compact(w, L.n, nullptr, w.wl[cur ^ 1], &n_wl, &c));
     moves += (int64_t)c;
     cur ^= 1;
-    if (getenv("SB2_TIMING") && getenv("SB2_VERBOSE")) fprintf(stderr, "[sb2 leiden]     sweep %d noskip=%d moves=%llu next=%d\n", sweep, noskip, c, n_wl);
+    if (w.verbose) fprintf(stderr, "[sb2 leiden]     sweep %d noskip=%d moves=%llu next=%d\n", sweep, noskip, c, n_wl);
     if (c == 0) {
       if (noskip) break;
       noskip = 1;  // confirm with a sweep in which every active vertex decides
@@ -596,7 +605,7 @@ int32_t local_move(Work& w, const Level& L, int32_t* comm, int64_t* moves_out) {
     prev_c = c;
   }
   *moves_out = moves;
-  if (getenv("SB2_TIMING")) fprintf(stderr, "[sb2 leiden]   local_move n=%d sweeps=%d moves=%lld\n", L.n, w.last_sweeps, (long long)moves);
+  if (w.timing) fprintf(stderr, "[sb2 leiden]   local_move n=%d sweeps=%d moves=%lld\n", L.n, w.last_sweeps, (long long)moves);
   return SB2_OK;
 }
 
@@ -618,7 +627,7 @@ int32_t refine(Work& w, const Level& L, const int32_t* comm, int32_t* ref, int64
     u64 c = 0;
     int32_t n_next = 0;
     SB2_TRY(compact(w, n_wl, w.wl[cur], w.wl[cur ^ 1], &n_next, &c));
-    if (getenv("SB2_TIMING")) fprintf(stderr, "[sb2 leiden]   refine n=%d round=%d singletons=%d merges=%llu\n", L.n, round, n_wl, c);
+    if (w.timing) fprintf(stderr, "[sb2 leiden]   refine n=%d round=%d singletons=%d merges=%llu\n", L.n, round, n_wl, c);
     cur ^= 1;
     n_wl = n_next;
     // the first rounds do nearly all the merging; stragglers (< 0.1 % of the vertices per round) simply stay
@@ -807,10 +816,12 @@ static int32_t leiden_core(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, con
   w.seed = (uint32_t)(seed ^ (seed >> 32));
   { const char* ex = getenv("SB2_LEIDEN_EXACT"); w.exact = ex && atoi(ex) > 0; }
   w.careful = n0 < 65536;
+  w.timing = getenv("SB2_TIMING") != nullptr;
+  w.verbose = w.timing && getenv("SB2_VERBOSE") != nullptr;
   SB2_TRY(scr.alloc(&w.K, (size_t)n0));
   SB2_TRY(scr.alloc(&w.csize, (size_t)n0));
-  SB2_TRY(scr.alloc(&w.hkeys, (size_t)std::max<int64_t>(nnz0, 1)));
-  SB2_TRY(scr.alloc(&w.hvals, (size_t)std::max<int64_t>(nnz0, 1)));
+  SB2_TRY(scr.alloc(&w.hkeys, (size_t)std::max<int64_t>(2 * nnz0, 1)));   // decide: 2 slots per arc; aggregation: 1
+  SB2_TRY(scr.alloc(&w.hvals, (size_t)std::max<int64_t>(2 * nnz0, 1)));
   SB2_TRY(scr.alloc(&w.target, (size_t)n0));
   SB2_TRY(scr.alloc(&w.tsingle, (size_t)n0));
   SB2_TRY(scr.alloc(&w.wl[0], (size_t)n0));
@@ -860,7 +871,9 @@ static int32_t leiden_core(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, con
         int64_t mv = 0;
         pt.reset();
         SB2_TRY(local_move(w, L, comm, &mv));
+        const double lm0 = t_lm;
         pt.lap(&t_lm);
+        if (w.timing) fprintf(stderr, "[sb2 leiden]   level n=%d local_move %.3f ms\n", L.n, t_lm - lm0);
         ++n_lm;
         pass_moves += mv;
         if (lev > 0) higher_moves += mv;
@@ -880,7 +893,9 @@ static int32_t leiden_core(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, con
         } else {
           SB2_TRY(refine(w, L, comm, ref, Kref, rsize));
         }
+        const double rf0 = t_rf;
         pt.lap(&t_rf);
+        if (w.timing) fprintf(stderr, "[sb2 leiden]   level n=%d refine %.3f ms\n", L.n, t_rf - rf0);
         // compact refined labels
         flag_nonempty_kernel<<<gridt(L.n), 256, 0, st>>>(L.n, rsize, flag);
         SB2_LAUNCH_CHECK(ctx);
@@ -888,6 +903,7 @@ static int32_t leiden_core(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, con
         int64_t nc64 = 0;
         SB2_CUDA(cudaMemcpyAsync(&nc64, scan_tmp + L.n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
         SB2_CUDA(cudaStreamSynchronize(st));
+        ++w.syncs;
         const int32_t nc = (int32_t)nc64;
         if (nc >= L.n) break;  // nothing merged: the aggregate would not shrink
         // ---- aggregate ----
@@ -898,6 +914,7 @@ static int32_t leiden_core(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, con
         int64_t eL = 0;
         SB2_CUDA(cudaMemcpyAsync(&eL, slice + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
         SB2_CUDA(cudaStreamSynchronize(st));
+        ++w.syncs;
         if (eL > 0) {
           agg_clear_kernel<<<gridt(eL), 256, 0, st>>>(eL, w.hkeys, w.hvals);
           SB2_LAUNCH_CHECK(ctx);
@@ -916,6 +933,7 @@ static int32_t leiden_core(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, con
         int64_t nnz_new = 0;
         SB2_CUDA(cudaMemcpyAsync(&nnz_new, indptr_new + nc, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
         SB2_CUDA(cudaStreamSynchronize(st));
+        ++w.syncs;
         int32_t* indices_new;
         int64_t *w_new, *k_new;
         SB2_TRY(lvl.alloc(&indices_new, (size_t)std::max<int64_t>(nnz_new, 1)));
@@ -950,8 +968,8 @@ static int32_t leiden_core(sb2_ctx* ctx, int64_t n, const int64_t* d_indptr, con
   SB2_TRY(quality_device(ctx, scr, n0, d_indptr, d_indices, wfx0, kfx0, total, resolution, d_membership, h_modularity, *h_n_comms));
   pt.lap(&t_fin);
   if (pt.on)
-    fprintf(stderr, "[sb2 leiden] n=%d passes=%d local_move %.1f ms (%d calls) refine %.1f ms aggregate %.1f ms finalize %.1f ms\n",
-            n0, passes, t_lm, n_lm, t_rf, t_agg, t_fin);
+    fprintf(stderr, "[sb2 leiden] n=%d passes=%d local_move %.1f ms (%d calls) refine %.1f ms aggregate %.1f ms finalize %.1f ms syncs=%lld\n",
+            n0, passes, t_lm, n_lm, t_rf, t_agg, t_fin, (long long)w.syncs);
   if (info) {
     info->passes = passes;
     info->levels = levels;
