@@ -613,6 +613,12 @@ KnnSwitches knn_switches() {
     const long v = strtol(e, &end, 10);
     s.near_tiles = (end != e && *end == '\0' && v >= 1 && v <= KNN_MAX_NEAR) ? (int)v : 0;
   }
+  if (const char* e = getenv("SB2_KNN_SPLIT")) s.split = strcmp(e, "principal") == 0 ? 1 : strcmp(e, "coord") == 0 ? 0 : -1;
+  if (const char* e = getenv("SB2_KNN_KD_WIDE")) {
+    char* end = nullptr;
+    const long long v = strtoll(e, &end, 10);
+    s.kd_wide = (end != e && *end == '\0' && v >= 1) ? (int64_t)v : 0;
+  }
   return s;
 }
 
@@ -772,8 +778,10 @@ int32_t screen_prep(KnnCall& c, Tier& t1, __half* A1, float* inv_s2, float* dnor
     for (int i = 0; i < 3; ++i) SB2_CUDA(cudaEventCreate(&ev[i]));
   SB2_TRY(c.evs.begin());
   if (ev[0]) SB2_CUDA(cudaEventRecord(ev[0], st));
+  SB2_CHECK_ARG(c.sw.split >= 0, "SB2_KNN_SPLIT must be principal or coord");
+  SB2_CHECK_ARG(c.sw.kd_wide >= 1, "SB2_KNN_KD_WIDE must be an integer >= 1");
   SB2_TRY(scr.alloc(&S.perm, (size_t)n_points));
-  SB2_TRY(knn_tc2_kd_order(ctx, c.d_x, n_points, d, S.perm));
+  SB2_TRY(knn_tc2_kd_order(ctx, c.d_x, n_points, d, c.sw.split == 0, c.sw.kd_wide, S.perm));
   if (c.q0 == 0 && n_query == n_points) {
     S.qloc = S.perm;
   } else {

@@ -7,6 +7,7 @@
 constexpr int EST_R = 6;           // chunk maxima an estimate keeps per (row, sub-list)
 constexpr int EST_STRIDE = 16;     // the estimate samples every 16th candidate tile
 constexpr int KNN_MAX_NEAR = 64;   // longest near list of the tile screen's short sweep (SB2_KNN_NEAR)
+constexpr int64_t KD_WIDE_MIN = 16384;   // kd order: segments from this length on are split by many CTAs each
 
 // float <-> unsigned with the same order (the kd order's radix select, the k-th largest proposal score)
 __device__ __forceinline__ uint32_t ord_bits(float x) {
@@ -30,6 +31,10 @@ struct KnnSwitches {
   bool int_scan = true;         // SB2_KNN_SCAN=float (false): the float max tree in the fast path of the sweep's examination
   int screen = -1;              // SB2_KNN_SCREEN=0: no tile screen; =1: screen at every size; unset: from 512 candidate tiles
   int near_tiles = 64;          // SB2_KNN_NEAR=1..KNN_MAX_NEAR: consecutive tiles of the kd order in the screen's short sweep
+  int split = 1;                // SB2_KNN_SPLIT=coord (0): the kd order splits on the coordinate of largest variance, not
+                                // the principal direction (=principal, 1); -1: an unknown value, which fails the screened call
+  int64_t kd_wide = KD_WIDE_MIN;   // SB2_KNN_KD_WIDE=n >= 1: the kd order's segment length from which many CTAs split one
+                                   // segment (the same permutation; tests force either path); 0: not an integer >= 1
 };
 
 // ---- tensor-core sweep (knn_tc2.cu): 128-query CTAs x 128-candidate tiles (wgmma N = 128), two consumer warpgroups,
@@ -71,8 +76,9 @@ int32_t knn_tc2_sweep(sb2_ctx* ctx, const KnnSwitches& sw, const KnnTc2Shape& sh
                       const __half* Bimg, int64_t n_points, int64_t n_query, int list_m, float* cand_score, int32_t* cand_idx,
                       double* issued_flops, const KnnTc2Lists* lists = nullptr);
 // ---- tile-compact order and tile screen (knn_tc2.cu) ----
-// perm[i] = the point at position i of the kd order (deterministic, depends on X alone)
-int32_t knn_tc2_kd_order(sb2_ctx* ctx, const float* d_x, int64_t n, int d, int32_t* perm);
+// perm[i] = the point at position i of the kd order (deterministic, depends on X alone); coord: split on coordinates
+// instead of principal directions; segments of wide_min points or more are split by many CTAs each
+int32_t knn_tc2_kd_order(sb2_ctx* ctx, const float* d_x, int64_t n, int d, bool coord, int64_t wide_min, int32_t* perm);
 // the query rows [q0, q0 + n_query) in perm's order: qloc[j] = local row, qpos[j] = its position in perm
 int32_t knn_tc2_restrict(sb2_ctx* ctx, const int32_t* perm, int64_t n, int64_t q0, int64_t n_query, int32_t* qloc, int32_t* qpos);
 // per tile of perm: cent[t * d ..] the centre (fp16-exact in the images' scale), rad[t] >= max |x - cent_t|

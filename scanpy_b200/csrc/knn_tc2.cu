@@ -622,18 +622,131 @@ knn_sweep2_kernel(const __half* __restrict__ Aimg, const __half* __restrict__ Bi
 // ------------------------------------------------------------------------------------------------
 // Tile-compact order and tile screen (SB2_KNN_SCREEN, on by default from 512 candidate tiles).
 //
-// kd order: the points are split recursively, each segment at a multiple of 128 points on the coordinate of largest
-// (sampled) variance, until every segment is one tile; knn.cu builds the fp16 images in that order, so each 128-point
+// kd order: the points are split recursively, each segment at a multiple of 128 points along its (sampled) principal
+// direction, until every segment is one tile; knn.cu builds the fp16 images in that order, so each 128-point
 // candidate tile and each 128-row query block is spatially compact.  Per tile a centre mu_t and a radius r_t bound every
 // point of the tile: |q - x| >= |q - mu_t| - r_t.  The screen scores every query row against every centre on the tensor
 // cores (the centres go through the same image builder) and keeps, per query block, the tiles for which some row has
 // |q - mu_t| - r_t <= u(q), where u(q) >= d_k(q) comes from a short sweep of the block's own neighbourhood.  A skipped
 // tile holds no point within u(q) of any row of the block; the re-score checks d_k(q) <= u(q) before it certifies a row.
-constexpr int KD_SAMPLES = 512;   // points per segment the split coordinate is chosen from
+constexpr int KD_SAMPLES = 512;   // points per segment the split direction is chosen from
 constexpr int KD_THREADS = 1024;
+constexpr int KD_POWER_ITERS = 12;                // power iterations of the split direction
+constexpr int KD_SAMPLE_SMEM = 200 * 1024;        // bytes of shared memory the direction's fp32 sample may take
+constexpr int KD_MAX_D = 150;                     // the kNN's largest d
 
-// segment s of a level = [seg[3s], seg[3s+2]), split at seg[3s+1]: its coordinate of largest variance over an evenly
-// spaced sample of its points (any choice is correct; the variance only makes the tiles tight)
+// Points in the sample of the direction kernel: KD_SAMPLES, fewer for d > 100 so the sample fits KD_SAMPLE_SMEM.
+constexpr int KD_DIR_PARTS = 256;   // the direction kernel's threads: partial sums of its scatter product, parts x d <= 256
+int kd_dir_samples(int d) { return std::min(KD_SAMPLES, KD_SAMPLE_SMEM / (4 * (d | 1))); }
+size_t kd_dir_smem(int d, int ns) { return (size_t)(3 * d + KD_DIR_PARTS + ns) * sizeof(double) + (size_t)ns * (d | 1) * sizeof(float); }
+
+// segment s of a level = [seg[3s], seg[3s+2]), split at seg[3s+1]: dir[s * (d + 1) ..] = its principal direction v (unit,
+// largest |v_j| positive) and the offset mu . v, from an evenly spaced sample of ns_max (or all) of its points, all in
+// fp64 and in a fixed order.  The sample is centred; KD_POWER_ITERS power iterations on its scatter start from the
+// coordinate of largest variance (a sample without spread keeps that coordinate).  Any direction is correct: it only
+// makes the tiles tight.
+__global__ void __launch_bounds__(256) kd_dir_kernel(const float* __restrict__ X, int d, const int32_t* __restrict__ P,
+                                                     const int32_t* __restrict__ seg, int ns_max, double* __restrict__ dir) {
+  extern __shared__ double kd_sm[];
+  const int ds = d | 1;   // odd row stride: a thread per sample row reads without bank conflicts
+  double* mu = kd_sm;     // [d]
+  double* v = mu + d;     // [d]
+  double* u = v + d;      // [d]
+  const int np = max(1, (int)blockDim.x / d);   // parts of the sample the scatter product is summed in
+  double* part = u + d;                         // [np][d], np d <= KD_DIR_PARTS
+  double* w = part + KD_DIR_PARTS;              // [ns]
+  const int64_t a = seg[3 * blockIdx.x], len = seg[3 * blockIdx.x + 2] - a;
+  const int ns = (int)min(len, (int64_t)ns_max);
+  float* xs = reinterpret_cast<float*>(w + ns);   // [ns][ds]
+  __shared__ double s_norm;
+  __shared__ int s_best;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int warp = tid >> 5, nwarps = blockDim.x >> 5;
+  for (int t0 = warp; t0 < ns; t0 += 4 * nwarps) {   // a warp per sample row, four rows in flight
+    int64_t row[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const int t = t0 + r * nwarps;
+      row[r] = t < ns ? (int64_t)P[a + t * len / ns] * d : -1;
+    }
+    for (int j = lane; j < d; j += 32)
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+        if (row[r] >= 0) xs[(t0 + r * nwarps) * ds + j] = X[row[r] + j];
+  }
+  __syncthreads();
+  for (int j = tid; j < d; j += blockDim.x) {
+    double s = 0.0;
+    for (int t = 0; t < ns; ++t) s += xs[t * ds + j];
+    mu[j] = s / ns;
+  }
+  __syncthreads();
+  for (int j = tid; j < d; j += blockDim.x) {
+    double s2 = 0.0;
+    for (int t = 0; t < ns; ++t) {
+      const double c = xs[t * ds + j] - mu[j];
+      s2 = fma(c, c, s2);
+    }
+    u[j] = s2;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int best = 0;
+    for (int j = 1; j < d; ++j)
+      if (u[j] > u[best]) best = j;
+    s_best = best;
+  }
+  __syncthreads();
+  for (int j = tid; j < d; j += blockDim.x) v[j] = j == s_best ? 1.0 : 0.0;
+  __syncthreads();
+  for (int it = 0; it < KD_POWER_ITERS; ++it) {
+    for (int t = tid; t < ns; t += blockDim.x) {   // w = (X_s - mu) v
+      double acc = 0.0;
+      for (int j = 0; j < d; ++j) acc = fma(xs[t * ds + j] - mu[j], v[j], acc);
+      w[t] = acc;
+    }
+    __syncthreads();
+    for (int e = tid; e < np * d; e += blockDim.x) {   // u = (X_s - mu)^T w, in np parts of the sample
+      const int h = e / d, j = e - h * d;
+      double acc = 0.0;
+      for (int t = h * ns / np; t < (h + 1) * ns / np; ++t) acc = fma(xs[t * ds + j] - mu[j], w[t], acc);
+      part[e] = acc;
+    }
+    __syncthreads();
+    if (tid < 32) {
+      double s2 = 0.0;
+      for (int j = lane; j < d; j += 32) {
+        double x = part[j];
+        for (int h = 1; h < np; ++h) x += part[h * d + j];
+        u[j] = x;
+        s2 = fma(x, x, s2);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+      if (lane == 0) s_norm = sqrt(s2);
+    }
+    __syncthreads();
+    const double nrm = s_norm;
+    if (!(nrm > 0.0) || !isfinite(nrm)) break;   // no spread in the sample: keep the current direction
+    for (int j = tid; j < d; j += blockDim.x) v[j] = u[j] / nrm;
+    __syncthreads();
+  }
+  if (tid == 0) {   // the sign: the largest |v_j| (the first of equals) positive
+    int best = 0;
+    for (int j = 1; j < d; ++j)
+      if (fabs(v[j]) > fabs(v[best])) best = j;
+    const double sg = v[best] < 0.0 ? -1.0 : 1.0;
+    double off = 0.0;
+    for (int j = 0; j < d; ++j) {
+      const double vj = sg * v[j];
+      dir[(int64_t)blockIdx.x * (d + 1) + j] = vj;
+      off = fma(mu[j], vj, off);
+    }
+    dir[(int64_t)blockIdx.x * (d + 1) + d] = off;
+  }
+}
+
+// SB2_KNN_SPLIT=coord: the segment's coordinate of largest variance over the same evenly spaced sample
 __global__ void __launch_bounds__(256) kd_axis_kernel(const float* __restrict__ X, int d, const int32_t* __restrict__ P,
                                                       const int32_t* __restrict__ seg, int32_t* __restrict__ axis) {
   __shared__ double var[256];
@@ -658,13 +771,43 @@ __global__ void __launch_bounds__(256) kd_axis_kernel(const float* __restrict__ 
   }
 }
 
-__global__ void kd_keys_kernel(const float* __restrict__ X, int d, const int32_t* __restrict__ P, const int32_t* __restrict__ seg,
-                               const int32_t* __restrict__ axis, uint32_t* __restrict__ key) {
+// the split keys: ord_bits(fp32(x . v - mu . v)) (the dot in fp64, in coordinate order), or with axis the coordinate itself
+__global__ void __launch_bounds__(256) kd_keys_kernel(const float* __restrict__ X, int d, const int32_t* __restrict__ P,
+                                                      const int32_t* __restrict__ seg, const double* __restrict__ dir,
+                                                      const int32_t* __restrict__ axis, uint32_t* __restrict__ key) {
+  __shared__ double v[KD_MAX_D + 1];
   const int64_t a = seg[3 * blockIdx.x], b = seg[3 * blockIdx.x + 2];
-  const int ax = axis[blockIdx.x];
-  for (int64_t i = a + (int64_t)blockIdx.y * blockDim.x + threadIdx.x; i < b; i += (int64_t)gridDim.y * blockDim.x)
-    key[i] = ord_bits(X[(int64_t)P[i] * d + ax]);
+  if (axis) {
+    const int ax = axis[blockIdx.x];
+    for (int64_t i = a + (int64_t)blockIdx.y * blockDim.x + threadIdx.x; i < b; i += (int64_t)gridDim.y * blockDim.x)
+      key[i] = ord_bits(X[(int64_t)P[i] * d + ax]);
+    return;
+  }
+  // a warp stages its 32 rows in shared memory, each row read whole by the warp, then a thread takes a row
+  extern __shared__ float kd_rows[];
+  const int lane = threadIdx.x & 31, ds = d | 1;
+  float* rows = kd_rows + (threadIdx.x >> 5) * 32 * ds;
+  for (int j = threadIdx.x; j <= d; j += blockDim.x) v[j] = dir[(int64_t)blockIdx.x * (d + 1) + j];
+  __syncthreads();
+  for (int64_t base = a + ((int64_t)blockIdx.y * blockDim.x + (threadIdx.x & ~31)); base < b; base += (int64_t)gridDim.y * blockDim.x) {
+    const int64_t i = base + lane;
+    const int32_t p = i < b ? P[i] : -1;
+#pragma unroll 8
+    for (int r = 0; r < 32; ++r) {
+      const int32_t pr = __shfl_sync(0xffffffffu, p, r);
+      if (pr >= 0)
+        for (int j = lane; j < d; j += 32) rows[r * ds + j] = X[(int64_t)pr * d + j];
+    }
+    __syncwarp();
+    if (i < b) {
+      double acc = 0.0;
+      for (int j = 0; j < d; ++j) acc = fma((double)rows[lane * ds + j], v[j], acc);
+      key[i] = ord_bits((float)(acc - v[d]));
+    }
+    __syncwarp();
+  }
 }
+size_t kd_keys_smem(int d) { return (size_t)256 * (d | 1) * sizeof(float); }   // a row per thread of 256
 
 // inclusive prefix sum of one value per thread over the CTA (in thread order); *total = the sum
 __device__ __forceinline__ int block_scan_incl(int v, int* wsum, int* total) {
@@ -692,57 +835,53 @@ __device__ __forceinline__ int block_scan_incl(int v, int* wsum, int* total) {
   return r;
 }
 
-// one CTA per segment: the m - a smallest keys (equal keys in position order) go to [a, m), the rest to [m, b), both
+// A split sends the m - a smallest keys of [a, b) (equal keys in position order) to [a, m), the rest to [m, b), both
 // in position order.  The pivot is found by a 4-pass radix select over the 32-bit keys (histogram counts aggregated per
 // warp: the top byte of nearby floats is nearly constant); the partition takes KD_PER consecutive keys per thread.
+// kd_split_kernel does a whole segment in one CTA; a wide level (segments longer than the wide threshold) spreads each
+// segment over CTAs of KD_CHUNK keys with the same arithmetic, so both give the same permutation.
 constexpr int KD_PER = 4;
-__global__ void __launch_bounds__(KD_THREADS) kd_split_kernel(const int32_t* __restrict__ seg, const uint32_t* __restrict__ key,
-                                                              const int32_t* __restrict__ P, int32_t* __restrict__ Pout) {
-  __shared__ unsigned hist[256];
-  __shared__ uint32_t s_prefix;
-  __shared__ int s_rank;
-  __shared__ int wsum[32];
-  const int64_t a = seg[3 * blockIdx.x], m = seg[3 * blockIdx.x + 1], b = seg[3 * blockIdx.x + 2];
+constexpr int KD_WIDE_THREADS = 256;
+constexpr int KD_CHUNK = KD_WIDE_THREADS * KD_PER * 4;   // keys per CTA of a wide level
+
+// adds to hist[bin] the keys of [lo, hi) that match prefix above `byte`, binned by `byte`
+__device__ __forceinline__ void kd_hist(const uint32_t* __restrict__ key, int64_t lo, int64_t hi, uint32_t prefix, int byte,
+                                        unsigned* hist) {
   const int lane = threadIdx.x & 31;
-  uint32_t prefix = 0;
-  int rank = (int)(m - a) - 1;   // sorted index of the pivot
-  for (int byte = 3; byte >= 0; --byte) {
-    for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0u;
-    __syncthreads();
-    const uint32_t hmask = byte == 3 ? 0u : (0xffffffffu << (8 * (byte + 1)));
-    for (int64_t base = a; base < b; base += blockDim.x) {
-      const int64_t i = base + threadIdx.x;
-      const uint32_t k = i < b ? key[i] : 0u;
-      const unsigned bin = (i < b && (k & hmask) == prefix) ? (k >> (8 * byte)) & 255u : 256u;
-      const unsigned peers = __match_any_sync(0xffffffffu, bin);
-      if (bin < 256u && lane == __ffs(peers) - 1) atomicAdd(&hist[bin], (unsigned)__popc(peers));
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      int r = rank, bin = 0;
-      for (; bin < 255; ++bin) {
-        if (r < (int)hist[bin]) break;
-        r -= (int)hist[bin];
-      }
-      s_prefix = prefix | ((uint32_t)bin << (8 * byte));
-      s_rank = r;
-    }
-    __syncthreads();
-    prefix = s_prefix;
-    rank = s_rank;
-    __syncthreads();
+  const uint32_t hmask = byte == 3 ? 0u : (0xffffffffu << (8 * (byte + 1)));
+  for (int64_t base = lo; base < hi; base += blockDim.x) {
+    const int64_t i = base + threadIdx.x;
+    const uint32_t k = i < hi ? key[i] : 0u;
+    const unsigned bin = (i < hi && (k & hmask) == prefix) ? (k >> (8 * byte)) & 255u : 256u;
+    const unsigned peers = __match_any_sync(0xffffffffu, bin);
+    if (bin < 256u && lane == __ffs(peers) - 1) atomicAdd(&hist[bin], (unsigned)__popc(peers));
   }
-  const uint32_t pivot = prefix;
-  const int eq_take = rank + 1;   // keys equal to the pivot that go left, the first ones in position order
-  int eq_before = 0, left_before = 0;
-  for (int64_t base = a; base < b; base += (int64_t)blockDim.x * KD_PER) {
+}
+
+// the bin of `byte` that holds sorted index *rank; *rank becomes the index within that bin
+__device__ __forceinline__ uint32_t kd_pick(const unsigned* hist, int byte, uint32_t prefix, int* rank) {
+  int r = *rank, bin = 0;
+  for (; bin < 255; ++bin) {
+    if (r < (int)hist[bin]) break;
+    r -= (int)hist[bin];
+  }
+  *rank = r;
+  return prefix | ((uint32_t)bin << (8 * byte));
+}
+
+// the partition of the keys [lo, hi) of segment [a, m, b) around pivot, given the keys equal to the pivot before lo
+// (eq_before) and the keys sent left before lo (left_before); eq_take of the equal keys go left
+__device__ __forceinline__ void kd_partition(const uint32_t* __restrict__ key, const int32_t* __restrict__ P, int32_t* __restrict__ Pout,
+                                             int64_t a, int64_t m, int64_t lo, int64_t hi, uint32_t pivot, int eq_take, int eq_before,
+                                             int left_before, int* wsum) {
+  for (int64_t base = lo; base < hi; base += (int64_t)blockDim.x * KD_PER) {
     const int64_t i0 = base + (int64_t)threadIdx.x * KD_PER;
     uint32_t k[KD_PER];
     int e_cnt = 0;
 #pragma unroll
     for (int j = 0; j < KD_PER; ++j) {
-      k[j] = i0 + j < b ? key[i0 + j] : 0u;
-      e_cnt += i0 + j < b && k[j] == pivot;
+      k[j] = i0 + j < hi ? key[i0 + j] : 0u;
+      e_cnt += i0 + j < hi && k[j] == pivot;
     }
     int tot;
     int eq_rank = eq_before + block_scan_incl(e_cnt, wsum, &tot) - e_cnt;
@@ -750,7 +889,7 @@ __global__ void __launch_bounds__(KD_THREADS) kd_split_kernel(const int32_t* __r
     unsigned lf = 0u;
 #pragma unroll
     for (int j = 0; j < KD_PER; ++j) {
-      const bool in = i0 + j < b, e = in && k[j] == pivot;
+      const bool in = i0 + j < hi, e = in && k[j] == pivot;
       lf |= (unsigned)(in && (k[j] < pivot || (e && eq_rank < eq_take))) << j;
       eq_rank += e;
     }
@@ -760,13 +899,124 @@ __global__ void __launch_bounds__(KD_THREADS) kd_split_kernel(const int32_t* __r
 #pragma unroll
     for (int j = 0; j < KD_PER; ++j) {
       const int64_t i = i0 + j;
-      if (i < b) {
+      if (i < hi) {
         const bool l = (lf >> j) & 1u;
         Pout[l ? a + left_ex : m + (i - a - left_ex)] = P[i];
         left_ex += l;
       }
     }
   }
+}
+
+// one CTA per segment
+__global__ void __launch_bounds__(KD_THREADS) kd_split_kernel(const int32_t* __restrict__ seg, const uint32_t* __restrict__ key,
+                                                              const int32_t* __restrict__ P, int32_t* __restrict__ Pout) {
+  __shared__ unsigned hist[256];
+  __shared__ uint32_t s_prefix;
+  __shared__ int s_rank;
+  __shared__ int wsum[32];
+  const int64_t a = seg[3 * blockIdx.x], m = seg[3 * blockIdx.x + 1], b = seg[3 * blockIdx.x + 2];
+  uint32_t prefix = 0;
+  int rank = (int)(m - a) - 1;   // sorted index of the pivot
+  for (int byte = 3; byte >= 0; --byte) {
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0u;
+    __syncthreads();
+    kd_hist(key, a, b, prefix, byte, hist);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      s_prefix = kd_pick(hist, byte, prefix, &rank);
+      s_rank = rank;
+    }
+    __syncthreads();
+    prefix = s_prefix;
+    rank = s_rank;
+    __syncthreads();
+  }
+  kd_partition(key, P, Pout, a, m, a, b, prefix, rank + 1, 0, 0, wsum);
+}
+
+// A wide level: CTA (c, s) holds the keys [a + c KD_CHUNK, a + (c + 1) KD_CHUNK) of segment s (gridDim.x covers the
+// longest segment; CTAs past the end return).  sel[2s] = the pivot's prefix so far, sel[2s + 1] = its rank within it;
+// hist [segments][256] is zero before each kd_wide_hist_kernel.
+__global__ void __launch_bounds__(KD_WIDE_THREADS) kd_wide_hist_kernel(const int32_t* __restrict__ seg, const uint32_t* __restrict__ key,
+                                                                       int byte, const uint32_t* __restrict__ sel, unsigned* __restrict__ hist) {
+  __shared__ unsigned h[256];
+  const int64_t a = seg[3 * blockIdx.y], b = seg[3 * blockIdx.y + 2];
+  const int64_t lo = a + (int64_t)blockIdx.x * KD_CHUNK;
+  if (lo >= b) return;
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) h[i] = 0u;
+  __syncthreads();
+  kd_hist(key, lo, min(b, lo + KD_CHUNK), byte == 3 ? 0u : sel[2 * blockIdx.y], byte, h);
+  __syncthreads();
+  for (int i = threadIdx.x; i < 256; i += blockDim.x)
+    if (h[i]) atomicAdd(&hist[(int64_t)blockIdx.y * 256 + i], h[i]);
+}
+
+// one CTA of 256 threads per segment: the pivot's next byte, then the histogram zeroed for the next pass
+__global__ void __launch_bounds__(256) kd_wide_pick_kernel(const int32_t* __restrict__ seg, int byte, uint32_t* __restrict__ sel,
+                                                           unsigned* __restrict__ hist) {
+  unsigned* hs = hist + (int64_t)blockIdx.x * 256;
+  if (threadIdx.x == 0) {
+    int rank = byte == 3 ? seg[3 * blockIdx.x + 1] - seg[3 * blockIdx.x] - 1 : (int)sel[2 * blockIdx.x + 1];
+    sel[2 * blockIdx.x] = kd_pick(hs, byte, byte == 3 ? 0u : sel[2 * blockIdx.x], &rank);
+    sel[2 * blockIdx.x + 1] = (uint32_t)rank;
+  }
+  __syncthreads();
+  hs[threadIdx.x] = 0u;
+}
+
+// per CTA of a wide level: cnt[2 (s gridDim.x + c)] = its keys below the pivot, [.. + 1] = its keys equal to it
+__global__ void __launch_bounds__(KD_WIDE_THREADS) kd_wide_count_kernel(const int32_t* __restrict__ seg, const uint32_t* __restrict__ key,
+                                                                        const uint32_t* __restrict__ sel, int* __restrict__ cnt) {
+  __shared__ int wsum[32];
+  const int64_t a = seg[3 * blockIdx.y], b = seg[3 * blockIdx.y + 2];
+  const int64_t lo = a + (int64_t)blockIdx.x * KD_CHUNK, hi = min(b, lo + KD_CHUNK);
+  if (lo >= b) return;
+  const uint32_t pivot = sel[2 * blockIdx.y];
+  int lt = 0, eq = 0;
+  for (int64_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+    const uint32_t k = key[i];
+    lt += k < pivot;
+    eq += k == pivot;
+  }
+  int tot_lt, tot_eq;
+  block_scan_incl(lt, wsum, &tot_lt);
+  block_scan_incl(eq, wsum, &tot_eq);
+  if (threadIdx.x == 0) {
+    int* c = cnt + 2 * ((int64_t)blockIdx.y * gridDim.x + blockIdx.x);
+    c[0] = tot_lt;
+    c[1] = tot_eq;
+  }
+}
+
+// one thread per segment: each CTA's keys equal to the pivot before it and keys sent left before it, in place of cnt
+__global__ void kd_wide_scan_kernel(const int32_t* __restrict__ seg, int n_seg, int chunks, const uint32_t* __restrict__ sel,
+                                    int* __restrict__ cnt) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n_seg) return;
+  const int64_t a = seg[3 * s], b = seg[3 * s + 2];
+  const int used = (int)((b - a + KD_CHUNK - 1) / KD_CHUNK);
+  const int eq_take = (int)sel[2 * s + 1] + 1;
+  int eq_before = 0, left_before = 0;
+  for (int c = 0; c < used; ++c) {
+    int* p = cnt + 2 * ((int64_t)s * chunks + c);
+    const int lt = p[0], eq = p[1];
+    p[0] = eq_before;
+    p[1] = left_before;
+    left_before += lt + max(0, min(eq, eq_take - eq_before));
+    eq_before += eq;
+  }
+}
+
+__global__ void __launch_bounds__(KD_WIDE_THREADS) kd_wide_scatter_kernel(const int32_t* __restrict__ seg, const uint32_t* __restrict__ key,
+                                                                          const uint32_t* __restrict__ sel, const int* __restrict__ cnt,
+                                                                          const int32_t* __restrict__ P, int32_t* __restrict__ Pout) {
+  __shared__ int wsum[32];
+  const int64_t a = seg[3 * blockIdx.y], m = seg[3 * blockIdx.y + 1], b = seg[3 * blockIdx.y + 2];
+  const int64_t lo = a + (int64_t)blockIdx.x * KD_CHUNK;
+  if (lo >= b) return;
+  const int* c = cnt + 2 * ((int64_t)blockIdx.y * gridDim.x + blockIdx.x);
+  kd_partition(key, P, Pout, a, m, lo, min(b, lo + KD_CHUNK), sel[2 * blockIdx.y], (int)sel[2 * blockIdx.y + 1] + 1, c[0], c[1], wsum);
 }
 
 __global__ void kd_iota_kernel(int32_t* __restrict__ P, int64_t n) {
@@ -1005,50 +1255,95 @@ int32_t knn_tc2_build_images(sb2_ctx* ctx, const KnnTc2Shape& sh, const float* d
 }
 
 
-int32_t knn_tc2_kd_order(sb2_ctx* ctx, const float* d_x, int64_t n, int d, int32_t* perm) {
+int32_t knn_tc2_kd_order(sb2_ctx* ctx, const float* d_x, int64_t n, int d, bool coord, int64_t wide_min, int32_t* perm) {
+  SB2_CHECK_ARG(d >= 1 && d <= KD_MAX_D, "kd order: d");
   cudaStream_t st = ctx->stream;
   // the segments of every level depend on n alone: [a, b) splits at a + 128 * floor(tiles / 2)
   std::vector<int32_t> segs;
-  std::vector<std::pair<size_t, int>> levels;   // (first segment, segments)
+  struct Level {
+    size_t first;   // first segment
+    int cnt;        // segments
+    int64_t len;    // the longest
+  };
+  std::vector<Level> levels;
   std::vector<std::pair<int64_t, int64_t>> cur{{0, n}}, nxt;
   int max_seg = 0;
+  int64_t wide_chunks = 0;   // largest segments x chunks of a wide level
   for (;;) {
     nxt.clear();
     const size_t first = segs.size() / 3;
+    int64_t len = 0;
     for (const auto& ab : cur) {
       if (ab.second - ab.first <= CN) continue;
       const int64_t m = ab.first + CN * (ceil_div64(ab.second - ab.first, CN) / 2);
       segs.insert(segs.end(), {(int32_t)ab.first, (int32_t)m, (int32_t)ab.second});
       nxt.push_back({ab.first, m});
       nxt.push_back({m, ab.second});
+      len = std::max(len, ab.second - ab.first);
     }
     const int cnt = (int)(segs.size() / 3 - first);
     if (cnt == 0) break;
-    levels.push_back({first, cnt});
+    levels.push_back({first, cnt, len});
     max_seg = max_seg > cnt ? max_seg : cnt;
+    if (len >= wide_min) wide_chunks = std::max(wide_chunks, (int64_t)cnt * ceil_div64(len, KD_CHUNK));
     cur.swap(nxt);
   }
   kd_iota_kernel<<<(unsigned)ceil_div64(n, 256), 256, 0, st>>>(perm, n);
   SB2_LAUNCH_CHECK(ctx);
   if (levels.empty()) return SB2_OK;
   ScratchScope scr(ctx);
-  int32_t *d_segs, *axis, *other;
-  uint32_t* key;
+  int32_t *d_segs, *axis = nullptr, *other;
+  double* dir = nullptr;
+  uint32_t *key, *sel = nullptr;
+  unsigned* hist = nullptr;
+  int* cnt = nullptr;
   SB2_TRY(scr.alloc(&d_segs, segs.size()));
-  SB2_TRY(scr.alloc(&axis, (size_t)max_seg));
+  if (coord) SB2_TRY(scr.alloc(&axis, (size_t)max_seg));
+  else SB2_TRY(scr.alloc(&dir, (size_t)max_seg * (d + 1)));
   SB2_TRY(scr.alloc(&other, (size_t)n));
   SB2_TRY(scr.alloc(&key, (size_t)n));
+  if (wide_chunks) {
+    SB2_TRY(scr.alloc(&sel, (size_t)max_seg * 2));
+    SB2_TRY(scr.alloc(&hist, (size_t)max_seg * 256));
+    SB2_TRY(scr.alloc(&cnt, (size_t)wide_chunks * 2));
+    SB2_CUDA(cudaMemsetAsync(hist, 0, (size_t)max_seg * 256 * sizeof(unsigned), st));   // each pick re-zeroes its own
+  }
+  const int ns_dir = kd_dir_samples(d);
+  if (!coord) {
+    SB2_CUDA(cudaFuncSetAttribute(kd_dir_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kd_dir_smem(d, ns_dir)));
+    SB2_CUDA(cudaFuncSetAttribute(kd_keys_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kd_keys_smem(d)));
+  }
   SB2_CUDA(cudaMemcpyAsync(d_segs, segs.data(), segs.size() * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   int32_t *src = perm, *dst = other;
   for (const auto& lv : levels) {
     const int32_t* sg = d_segs + lv.first * 3;
-    const unsigned ns = (unsigned)lv.second;
+    const unsigned ns = (unsigned)lv.cnt;
     SB2_CUDA(cudaMemcpyAsync(dst, src, (size_t)n * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));   // unsplit segments
-    kd_axis_kernel<<<ns, 256, 0, st>>>(d_x, d, src, sg, axis);
+    if (coord) {
+      kd_axis_kernel<<<ns, 256, 0, st>>>(d_x, d, src, sg, axis);
+    } else {
+      const int ns_lv = (int)std::min<int64_t>(lv.len, ns_dir);
+      kd_dir_kernel<<<ns, 256, kd_dir_smem(d, ns_lv), st>>>(d_x, d, src, sg, ns_dir, dir);
+    }
     SB2_LAUNCH_CHECK(ctx);
-    kd_keys_kernel<<<dim3(ns, (unsigned)ceil_div64(2048, ns)), 256, 0, st>>>(d_x, d, src, sg, axis, key);
+    kd_keys_kernel<<<dim3(ns, (unsigned)ceil_div64(2048, ns)), 256, coord ? 0 : kd_keys_smem(d), st>>>(d_x, d, src, sg, dir, axis, key);
     SB2_LAUNCH_CHECK(ctx);
-    kd_split_kernel<<<ns, KD_THREADS, 0, st>>>(sg, key, src, dst);
+    if (lv.len >= wide_min) {
+      const dim3 grid((unsigned)ceil_div64(lv.len, KD_CHUNK), ns);
+      for (int byte = 3; byte >= 0; --byte) {
+        kd_wide_hist_kernel<<<grid, KD_WIDE_THREADS, 0, st>>>(sg, key, byte, sel, hist);
+        SB2_LAUNCH_CHECK(ctx);
+        kd_wide_pick_kernel<<<ns, 256, 0, st>>>(sg, byte, sel, hist);
+        SB2_LAUNCH_CHECK(ctx);
+      }
+      kd_wide_count_kernel<<<grid, KD_WIDE_THREADS, 0, st>>>(sg, key, sel, cnt);
+      SB2_LAUNCH_CHECK(ctx);
+      kd_wide_scan_kernel<<<(unsigned)ceil_div64(ns, 128), 128, 0, st>>>(sg, (int)ns, (int)grid.x, sel, cnt);
+      SB2_LAUNCH_CHECK(ctx);
+      kd_wide_scatter_kernel<<<grid, KD_WIDE_THREADS, 0, st>>>(sg, key, sel, cnt, src, dst);
+    } else {
+      kd_split_kernel<<<ns, KD_THREADS, 0, st>>>(sg, key, src, dst);
+    }
     SB2_LAUNCH_CHECK(ctx);
     int32_t* t = src; src = dst; dst = t;
   }
