@@ -386,6 +386,25 @@ int32_t sb2_aggregate_median(sb2_ctx* ctx, int32_t n_seg, const int64_t* h_seg_r
                              int32_t g, int32_t is_f64, const void* d_x, const int64_t* d_indptr,
                              const int32_t* d_indices, const void* d_data, const int64_t* d_order, void* d_out);
 
+/* ---- sc.pp.scrublet / sc.pp.scrublet_simulate_doublets (src/scanpy/preprocessing/_scrublet/core.py:188-238, 313-386;
+ * csrc/scrublet.cu) ----
+ * sb2_scrublet_pair_sums  <- scipy's canonical `x[p0] + x[p1]` for every row pair of d_pairs int64 [n_sim x 2] of the
+ *                            observed CSR (int64 indptr, sorted unique int32 indices, float32 data): d_out_indptr int64
+ *                            [n_sim + 1]; d_out_indices / d_out_data hold at least Σ_s (nnz(p0) + nnz(p1)) entries, of
+ *                            which d_out_indptr[n_sim] are written.  Entries whose fp32 sum is 0 are dropped.
+ * sb2_knn_label_count_f32 <- the k-neighbour label count of Scrublet's classifier over the points d_x [n x d] fp32
+ *                            row-major (1 <= k <= n < 2^31, d <= 256, |x| <= 2^55 and finite).  Point i's neighbour set
+ *                            is i plus its k - 1 nearest other points in (fp64 squared distance, id) order, the fp64
+ *                            squared distance summed over the columns in order with every operation rounded.
+ *                            d_count int32 [n] = members with id >= n_first; d_kth fp64 [n] = the fp64 distance of the
+ *                            (k - 1)-th other member (0 when k = 1); d_ids int32 [n x k] (may be NULL) = the set, i first,
+ *                            the rest unordered. */
+int32_t sb2_scrublet_pair_sums(sb2_ctx* ctx, int64_t n_obs, const int64_t* d_indptr, const int32_t* d_indices,
+                               const float* d_data, int64_t n_sim, const int64_t* d_pairs, int64_t* d_out_indptr,
+                               int32_t* d_out_indices, float* d_out_data);
+int32_t sb2_knn_label_count_f32(sb2_ctx* ctx, int64_t n_points, int32_t d, const float* d_x, int64_t n_first,
+                                int32_t k, int32_t* d_count, double* d_kth, int32_t* d_ids);
+
 /* ---- extreme eigenpairs of diag(s) A diag(s), A symmetric fp32 CSR (csrc/eigs.cu: thick-restart Lanczos, fp64) ----
  * Replaces `scipy.sparse.linalg.eigsh(matrix.astype(float64), k=n_comps, which='LM', v0=...)` in
  * Neighbors.compute_eigen (src/scanpy/neighbors/__init__.py:832-884; sc.tl.diffmap) and the eigsh of umap's spectral

@@ -166,6 +166,10 @@ SIGNATURES = {
                                         c_void_p]),
     "sb2_aggregate_median": (c_int32, [c_void_p, c_int32, c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p,
                                        c_void_p, c_void_p, c_void_p, c_void_p]),
+    "sb2_scrublet_pair_sums": (c_int32, [c_void_p, c_int64, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p,
+                                         c_void_p, c_void_p]),
+    "sb2_knn_label_count_f32": (c_int32, [c_void_p, c_int64, c_int32, c_void_p, c_int64, c_int32, c_void_p, c_void_p,
+                                          c_void_p]),
 }
 
 _lib = None

@@ -122,20 +122,12 @@ def _col_mean_var_expm1(x_log, log_scale: float):
     return mean, var
 
 
-def highly_variable_genes(adata, *, layer=None, n_top_genes: int | None = None, min_disp: float = 0.5,
-                          max_disp: float = np.inf, min_mean: float = 0.0125, max_mean: float = 3, span: float = 0.3,
-                          n_bins: int = 20, flavor: str = "seurat", subset: bool = False, inplace: bool = True,
-                          batch_key=None, filter_unexpressed_genes=None, check_values: bool = True):
-    """Annotate highly variable genes (signature of `scanpy.pp.highly_variable_genes`; flavor='seurat' only)."""
-    if flavor != "seurat":
-        raise NotImplementedError(f"flavor={flavor!r}: only 'seurat' is implemented in scanpy_b200")
-    if batch_key is not None or layer is not None:
-        raise NotImplementedError("`batch_key`/`layer` are not implemented in scanpy_b200.pp.highly_variable_genes")
-    start = log_start("extracting highly variable genes")
-    if n_top_genes is not None and (min_disp, max_disp, min_mean, max_mean) != (0.5, np.inf, 0.0125, 3):
-        warn("If you pass `n_top_genes`, all cutoffs are ignored.", UserWarning)
-    base = adata.uns.get("log1p", {}).get("base")
-    mean, var = _col_mean_var_expm1(adata.X, 1.0 if base is None else float(np.log(base)))
+def _hvg_seurat_frame(x_log, base, *, n_top_genes: int | None = None, min_disp: float = 0.5, max_disp: float = np.inf,
+                      min_mean: float = 0.0125, max_mean: float = 3, n_bins: int = 20) -> pd.DataFrame:
+    """The seurat flavour's per-gene table of a log1p'd matrix (natural log when `base` is None): means, dispersions,
+    dispersions_norm and highly_variable, on a RangeIndex.  Shared by `highly_variable_genes` and `pp.scrublet`, which
+    selects genes on a log1p copy of its matrix."""
+    mean, var = _col_mean_var_expm1(x_log, 1.0 if base is None else float(np.log(base)))
     # --- per-gene logic, verbatim from _highly_variable_genes.py:347-385,452-560 ---
     mean[mean == 0] = 1e-12
     dispersion = var / mean
@@ -166,7 +158,24 @@ def highly_variable_genes(adata, *, layer=None, n_top_genes: int | None = None, 
         v = np.sort(v)[::-1]
         hv = np.nan_to_num(dn, nan=-np.inf) >= v[n - 1]
     df["highly_variable"] = hv
-    df = df.drop(columns=["mean_bin"])
+    return df.drop(columns=["mean_bin"])
+
+
+def highly_variable_genes(adata, *, layer=None, n_top_genes: int | None = None, min_disp: float = 0.5,
+                          max_disp: float = np.inf, min_mean: float = 0.0125, max_mean: float = 3, span: float = 0.3,
+                          n_bins: int = 20, flavor: str = "seurat", subset: bool = False, inplace: bool = True,
+                          batch_key=None, filter_unexpressed_genes=None, check_values: bool = True):
+    """Annotate highly variable genes (signature of `scanpy.pp.highly_variable_genes`; flavor='seurat' only)."""
+    if flavor != "seurat":
+        raise NotImplementedError(f"flavor={flavor!r}: only 'seurat' is implemented in scanpy_b200")
+    if batch_key is not None or layer is not None:
+        raise NotImplementedError("`batch_key`/`layer` are not implemented in scanpy_b200.pp.highly_variable_genes")
+    start = log_start("extracting highly variable genes")
+    if n_top_genes is not None and (min_disp, max_disp, min_mean, max_mean) != (0.5, np.inf, 0.0125, 3):
+        warn("If you pass `n_top_genes`, all cutoffs are ignored.", UserWarning)
+    base = adata.uns.get("log1p", {}).get("base")
+    df = _hvg_seurat_frame(adata.X, base, n_top_genes=n_top_genes, min_disp=min_disp, max_disp=max_disp,
+                           min_mean=min_mean, max_mean=max_mean, n_bins=n_bins)
     df.index = adata.var.index
     log_done(start)
     if inplace:

@@ -20,6 +20,7 @@ from ._qc import calculate_qc_metrics, filter_cells, filter_genes  # noqa: F401
 from ._regress import regress_out  # noqa: F401
 from ._combat import combat  # noqa: F401
 from ._harmony import harmony_integrate  # noqa: F401
+from ._scrublet import scrublet, scrublet_simulate_doublets  # noqa: F401
 from ._compat import (MiniAnnData, accepts_legacy_random_state, as_csr_f32, is_anndata_like, log_done, log_start,
                       meta_random_state, seed_from_rng, settings, warn)
 
